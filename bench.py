@@ -1,13 +1,16 @@
 #!/usr/bin/env python
-"""bench.py -- VITA omni forward path on B200: 1 image + 10 s audio + text prefill -> 256-token greedy decode,
-Mixtral-8x7B geometry (32 layers, bf16, random-init weights, synthetic inputs).
+"""bench.py -- VITA omni forward path on H100: 1 image + 10 s audio + text prefill -> 256-token greedy decode,
+Mixtral-8x7B geometry cut to the 24 layers whose bf16 weights (70 GB) fit one 80 GB H100 (random-init weights,
+synthetic inputs; --layers 32 is the full stack, for expert-parallel runs over several GPUs).
 
     python bench.py --gpus 1 --steps K --warmup W              # this repo's CUDA path
     python bench.py --impl reference --gpus 1 --steps K ...    # the reference algorithm on the host CPU (oracle port)
     torchrun --nproc-per-node N bench.py --gpus N ...          # N independent replicas (request parallel, weak scaling)
 
-A step = one complete generate(): InternViT + Whale encoders, splice, 32-layer sparse-MoE prefill, 256 decode steps.
-Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for every field.
+A step = one complete generate(): InternViT + Whale encoders, splice, sparse-MoE prefill, 256 decode steps.
+Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for every field.  --dump-outputs DIR writes the ids the
+last timed step generated and, from one more untimed pass over the same inputs, the spliced embeddings and the last-row
+prefill logits, as float32 DIR/<name>.npy.
 """
 from __future__ import annotations
 
@@ -40,7 +43,7 @@ def peaks():
         d = json.loads(p.read_text())
         return dict(hbm_gbs=float(d["hbm_gbs"]), tflops=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, tflops=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, tflops=989.0, source="NVIDIA H100 SXM data sheet (700 W), not a measurement")
 
 
 def prefill_flops(S: int, cfg) -> float:
@@ -163,7 +166,7 @@ def cpu_reference_state(layers_cpu: int):
 
 def cpu_reference_sample(cfg_full, layers_cpu: int, n_decode: int, threads: int, built=None, repeats: int = 3):
     """One bounded sample of the bench workload on the host: encoders + splice, S-token prefill, `n_decode` greedy
-    steps; each phase is the best of `repeats` runs (perf_counter), the layer stack extrapolated x(32 / layers_cpu)."""
+    steps; each phase is the best of `repeats` runs (perf_counter), the layer stack extrapolated to the full depth."""
     from oracle import vita_oracle as O
     torch.set_num_threads(threads)
     state, cfg = built if built is not None else cpu_reference_state(layers_cpu)
@@ -197,8 +200,8 @@ def cpu_reference_sample(cfg_full, layers_cpu: int, n_decode: int, threads: int,
 
 def pick_cpu_threads() -> int:
     """Fixed rule (recorded in the JSON line): 16 threads, or all of them on a smaller host.  The oracle is plain
-    torch on CPU and this workload is many small ops; on the 128-thread GPU box all threads are ~10x slower than 8-16
-    (round 1 measured 31 s vs 2.5 s for the encoders), and probing per run made the baseline swing by +-40 %."""
+    torch on CPU and this workload is many small ops, which run slower on very many threads than on 8-16; probing per
+    run would make the baseline swing."""
     return min(16, os.cpu_count() or 1)
 
 
@@ -246,8 +249,8 @@ def workload_config(cfg, args, n):
                         f"S={spliced_len(cfg)} omni prefill -> {args.new_tokens}-token greedy decode, bs=1 per GPU",
             "geometry": f"Mixtral-8x7B ({cfg.llm.num_hidden_layers} layers, H=4096, I=14336, 8 experts top-2, "
                         "V=51760) + InternViT-300M + Whale, random init",
-            "parallelism": f"replica x{n} (request parallel; the model fits one 180 GB B200)",
-            "l2_policy": "inputs larger than L2 (93.7 GB of weights streamed every step)"}
+            "parallelism": f"replica x{n} (request parallel; the {cfg.llm.num_hidden_layers}-layer model fits one 80 GB H100)",
+            "l2_policy": "inputs larger than L2 (the weights are streamed every step)"}
 
 
 # ================================================================================================ expert-parallel record
@@ -452,6 +455,20 @@ def run_b200(args):
     launches = eager_launches + args.steps * NT * llm.launches_per_decode_step + enc_replayed
     toks = llm.generated_tokens(0)
     assert len(toks) == NT and all(0 <= t < cfg.llm.vocab_size for t in toks)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        # the ids the last timed step generated (what a caller of generate() receives) ...
+        np.save(os.path.join(args.dump_outputs, "generated_ids.npy"), np.asarray(toks, dtype=np.float32))
+        # ... and, from one more untimed pass over the same inputs (the timed path itself stays as it is without the
+        # option), the spliced embeddings the encoders produce and the last-row logits of the prefill: S x H and 1 x V
+        # values, 8.5 MB as float32.  prefill() uses its input as the residual stream, hence the clone.
+        emb_d, lens_d = model._embeds_for(ids, images_d, {"audios": feats_d, "lengths": lengths})
+        np.save(os.path.join(args.dump_outputs, "embeds.npy"), emb_d[0, : lens_d[0]].float().cpu().numpy())
+        llm.reset()
+        llm.prefill(emb_d[0, : lens_d[0]].clone(), slot=0, want_last_logits=True)
+        np.save(os.path.join(args.dump_outputs, "prefill_logits.npy"), llm.d_logits[:1].float().cpu().numpy())
+        llm.reset()
 
     # ---- e2e: the public generate() with HOST inputs (pinned), H2D + D2H inside the timed region ------------
     barrier()
@@ -512,7 +529,7 @@ def run_b200(args):
             ops.decode_tc_moe_gate_up(llm.d_h[:1], lw[li]["ln2"], lw[li]["gate"], lw[li]["w13"], llm.d_ids[:1],
                                       llm.d_w[:1], llm.d_act[:1], llm.tc_ws, c.rms_norm_eps)
 
-    # one launch per layer (32 different 470 MB weight sets, far larger than L2), back to back on the stream;
+    # one launch per layer (every layer its own 470 MB weight set, far larger than L2), back to back on the stream;
     # average duration = elapsed / launches
     launch_all()
     torch.cuda.synchronize()
@@ -560,14 +577,12 @@ def run_b200(args):
                         "encoders_tflops": encoder_flops(cfg) / (enc_ms / 1e3) / 1e12},
             "roofline": {"kernel": roof_kernel, "how": roof_note, "bound": "hbm", "achieved": gu_bytes / 1e9 / (gu_ms / 1e3),
                          "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": gu_bytes / 1e9 / (gu_ms / 1e3) / pk["hbm_gbs"],
-                         "traffic": ncu_traffic_bytes(roof_kernel), "bytes_per_launch": gu_bytes,
-                         "us_per_launch": gu_ms * 1e3, "peak_source": pk["source"],
-                         "traffic_source": "profiles/r02_prof_tc_gateup_full.md (ncu --set full, one launch, "
-                                           "dram__bytes_read.sum + dram__bytes_write.sum)"},
+                         "bytes_per_launch": gu_bytes, "us_per_launch": gu_ms * 1e3, "peak_source": pk["source"]},
             "prefill_long": None if long_ms is None else {
                 "S": S_LONG, "ms": long_ms, "tflops": prefill_flops(S_LONG, cfg) / (long_ms / 1e3) / 1e12,
                 "tensor_frac": prefill_flops(S_LONG, cfg) / (long_ms / 1e3) / 1e12 / pk["tflops"],
-                "note": "Mixtral prefill only, 32 layers, one GPU, random embeddings (BASELINE configs[3] length)"},
+                "note": f"Mixtral prefill only, {cfg.llm.num_hidden_layers} layers, one GPU, random embeddings "
+                        "(BASELINE configs[3] length)"},
             "e2e": {"value": world * NT / (e2e_ms / 1e3), "unit": UNIT,
                     "h2d_bytes_per_step": images_h.numel() * 4 + feats_h.numel() * 4 + ids.numel() * 8,
                     "d2h_bytes_per_step": NT * 4 + (TEXT_TOKENS + NT) * 8, "ms_per_step": e2e_ms,
@@ -626,28 +641,17 @@ def run_b200(args):
             pass
 
 
-def ncu_traffic_bytes(kernel_name: str):
-    """DRAM bytes of one launch of the roofline kernel, from the committed ncu --set full summary (None if the active
-    decode path is not the profiled kernel or the summary is missing)."""
-    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "r02_prof_tc_gateup_full.md")
-    if "TcGateUpOp" not in kernel_name or not os.path.exists(path):
-        return None
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    tot = 0.0
-    for ln in open(path):
-        c = [x.strip() for x in ln.strip().strip("|").split("|")]
-        if len(c) >= 3 and c[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum") and c[2] in unit:
-            tot += float(c[1]) * unit[c[2]]
-    return tot or None
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--layers", type=int, default=32)
+    ap.add_argument("--layers", type=int, default=24,
+                    help="Mixtral layers; 24 (70 GB of bf16 weights) is what one 80 GB H100 holds, 32 is the full model")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the generated ids of the last one (and embeddings / prefill logits of one "
+                         "more untimed pass) as float32 DIR/<name>.npy")
     ap.add_argument("--new-tokens", type=int, default=256)
     ap.add_argument("--cpu-layers", type=int, default=2)
     ap.add_argument("--cpu-decode-tokens", type=int, default=4)

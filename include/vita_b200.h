@@ -1,4 +1,4 @@
-/* libvita_b200.so -- C ABI of the B200-native (sm_100a) kernels behind VITA's omni-modal prefill + decode forward.
+/* libvita_b200.so -- C ABI of the H100-native (sm_90a) kernels behind VITA's omni-modal prefill + decode forward.
  *
  * The reference (VITA-MLLM/VITA) is pure Python and has no FFI of its own: every GPU op is reached through
  * torch / transformers / flash-attn / vLLM wheels.  This header is therefore the boundary a maintainer binds with
@@ -12,7 +12,7 @@
  *   - `stream` is a cudaStream_t passed as void* (NULL = legacy default stream);
  *   - every function returns VITA_OK (0) or a negative error code and records a message retrievable with
  *     vita_last_error(); nothing allocates device memory (workspaces are passed in);
- *   - there is no CPU fallback: on a machine without an sm_100 GPU the launches fail with VITA_ERR_CUDA.
+ *   - there is no CPU fallback: on a machine without an sm_90 GPU the launches fail with VITA_ERR_CUDA.
  */
 #ifndef VITA_B200_H
 #define VITA_B200_H
@@ -54,7 +54,7 @@ int vita_chain_begin(uint64_t* mem, int64_t n_links);
 int vita_chain_end(void);
 
 /* ---- dense linear:  C[M,N] = residual + colscale * act(A[M,K] . B[N,K]^T + bias) ----------------------------
- * tcgen05 / TMEM / TMA GEMM.  Replaces nn.Linear -> cuBLAS at
+ * wgmma / TMA GEMM.  Replaces nn.Linear -> cuBLAS at
  *   internvit/modeling_intern_vit.py:180 (qkv), :192 (proj, with ls1 + residual :245-247),
  *   :214,216 (fc1+GELU, fc2 with ls2 + residual :249-251); multimodal_projector/builder.py:164-168;
  *   whale/module/layer/attention.py:371-373,381,419; :145-147; component/subsampling.py:34;
@@ -243,9 +243,9 @@ int vita_decode_router(const void* h, const void* norm_w, const void* gate_w, vo
 int vita_decode_slots(const int32_t* cur_pos, const int32_t* block_table, int32_t* slots, int64_t B, int64_t page_size,
                       int64_t max_pages, void* stream);
 int vita_argmax_rows(const void* logits, uint64_t* best, int64_t B, int64_t V, void* stream);
-/* ---- greedy decode step on the tensor cores (tcgen05 swap-AB GEMV, stream-K) ---------------------------------
+/* ---- greedy decode step on the tensor cores (wgmma swap-AB GEMV, stream-K) ---------------------------------
  * Every linear of the decode step as a weight-streaming GEMV on the tensor cores: the weight tile is the M operand of
- * tcgen05.mma and the activation vector as row 0 of a 16-wide N operand; (row-block, k-block) units are split evenly
+ * wgmma and the activation vector as row 0 of a 16-wide N operand; (row-block, k-block) units are split evenly
  * over all SMs and combined through `workspace` (vita_decode_tc_workspace_bytes, zero-initialised once, shared by all
  * five calls; ws_row_blocks = the max_row_blocks it was sized for): K-partials travel as 64-bit {value, tag} words,
  * the CTA that ends on a row block adds them in slot order (deterministic) and clears the tags.  K multiples of 64.

@@ -57,7 +57,7 @@ def cmd_search(args):
     (if that reproduces the 32 tokens) in numerically distinct variants of itself: exp2 without the polynomial chunk,
     the narrow router summation order, a cos/sin table computed by another libm.  A seed that survives all of them is
     reproducible at bf16 precision for a reason (its decisions have real margins), not by a coin flip: a random-init MoE
-    turns an ulp into another trajectory at most seeds (profiles/r02_pr1_seed_search.json)."""
+    turns an ulp into another trajectory at most seeds."""
     on_gpu = torch.cuda.is_available()      # a GPU makes a candidate cost ~0.2 s instead of ~35 s; the CPU works too
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False

@@ -13,7 +13,7 @@ non-degenerate and a seed chosen once and recorded:
 * the router weights are scaled x8 (a power of two: exact in bf16).  Two bf16 effects compete: a rank-2 / rank-3
   near-tie flips an expert (frequency ~3 % of all decisions whatever the scale; harm = the second expert's weight, large
   for soft routers), and the noise of the top-1 / top-2 logit difference moves the mixing weights (harm ~ scale).  Round 2
-  measured both ends on the GPU (profiles/r02_pr1_seed_search.json): x1 and x128 reproduce an fp32 trajectory less often
+  measured both ends on the GPU: x1 and x128 reproduce an fp32 trajectory less often
   than x8 / x16, where a flipped second expert mostly carries a few percent of weight and the weight noise stays ~1.5 %;
 * everything else is `vita_b200.weights.synthetic_state` (std 0.02 matrices, 1 +- 0.1 norm gains), seed 0;
 * the prompt seed: `make_golden_pr1.py search` walks the seeds, keeps those whose 33 logit rows are clear of near-ties

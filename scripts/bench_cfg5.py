@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """BASELINE configs[4] on one GPU: B concurrent audio queries (10 s audio + short prompt each), paged-KV batched
-greedy decode; reports p50 / p99 inter-token latency and tokens/s.  (8 x B200 = 8 such replicas.)
+greedy decode; reports p50 / p99 inter-token latency and tokens/s.  (8 x H100 = 8 such replicas.)
 
     python scripts/bench_cfg5.py [--batch 16] [--new-tokens 256] [--layers 32]
     python scripts/bench_cfg5.py --arrivals 12          # staggered arrivals (mean gap in decode steps) through the

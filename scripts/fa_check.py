@@ -1,4 +1,4 @@
-"""Bring-up / benchmark aid for the tcgen05 FlashAttention (flash_tc.cu): one case per process so that a device trap
+"""Bring-up / benchmark aid for the wgmma FlashAttention (flash_tc.cu): one case per process so that a device trap
 in one case does not take the others down.  usage: python scripts/fa_check.py <kind> <S> [bench]
 kind: mix (causal GQA 32/8 x 128), vit (16 x 64, batch 8), whale (16 heads, 128/64, padded batch of 2)"""
 import sys

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Times the tcgen05 GEMM on the shapes of the BASELINE prefill (S=506 and S=4096) with both tile widths."""
+"""Times the wgmma GEMM on the shapes of the BASELINE prefill (S=506 and S=4096) with both tile widths."""
 import json, os, subprocess, sys
 from pathlib import Path
 ROOT = Path(__file__).resolve().parent.parent

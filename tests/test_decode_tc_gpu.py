@@ -1,4 +1,4 @@
-"""Decode-step linears on tcgen05 (swap-AB GEMV, stream-K with tagged partial slots) vs the oracle's functions.
+"""Decode-step linears on wgmma (swap-AB GEMV, stream-K with tagged partial slots) vs the oracle's functions.
 Each kernel is launched twice on the same workspace to exercise the self-clearing slot tags."""
 import pytest
 import torch

@@ -1,9 +1,9 @@
-"""Replays the call sequence of the reference demo (/root/reference/video_audio_demo.py:163-276) against the drop-in
+"""Replays the call sequence of the reference demo (video_audio_demo.py:163-276) against the drop-in
 surface on a synthetic tiny model: CUDA `input_ids`, fp16 `audios`, `output_scores=True, return_dict_in_generate=True,
 max_new_tokens=..., stopping_criteria=[KeywordsStoppingCriteria(...)]` and the `input_ids != output_ids[:, :L]` check.
 
 The tokenizer and the stopping-criteria class are the reference's own host-side Python (out of scope for the kernel
-tier, absent on the GPU box); the stand-ins below restate their behaviour (vita/util/mm_utils.py:121-155) so that the
+tier); the stand-ins below restate their behaviour (vita/util/mm_utils.py:121-155) so that the
 test exercises exactly what `generate()` has to support."""
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (vita_gemm_bf16 + grouped MoE variants) against the oracle's `linear` on the same bf16 inputs."""
+"""wgmma GEMM (vita_gemm_bf16 + grouped MoE variants) against the oracle's `linear` on the same bf16 inputs."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -53,12 +53,15 @@ def test_gemm_model_shapes():
     _run(256, 4096, 4096, bias=True, act=1)      # projector
 
 
-def test_gemm_tail_split_shapes():
-    # tiles of the last partial wave are cut along N (gemm_sm100.cu Sched): 148-SM tile counts with a short tail
-    _run(2048, 5120, 512, bias=True)             # 256-wide: 320 tiles = 2 waves + 24 -> pieces of 64 columns
-    _run(2048, 3328, 512, residual=True)         # 208 tiles = 1 wave + 60 -> pieces of 128 columns
-    _run(1025, 3072, 256, bias=True, act=1)      # 128-wide: 216 tiles = 1 wave + 68 -> pieces of 64 columns
-    _run(4096, 4096, 1024, residual=True)        # o_proj at S=4096: 512 tiles = 3 waves + 68
+def test_gemm_tail_split_shapes(monkeypatch):
+    # tiles of the last partial wave are cut along N (gemm_sm90.cu Sched); tile counts as chosen on 132 SMs
+    _run(2048, 5120, 512, bias=True)             # 256-wide: 320 tiles = 2 waves + 56 -> pieces of 128 columns
+    _run(2048, 2560, 512, bias=True)             # 160 tiles = 1 wave + 28 -> pieces of 64 columns
+    _run(2048, 3328, 512, residual=True)         # 208 tiles = 1 wave + 76: too many for a cut, whole tiles
+    _run(1025, 3072, 256, bias=True, act=1)      # 108 tiles of 256 columns, one partial wave, ragged last row tile
+    _run(4096, 4096, 1024, residual=True)        # o_proj at S=4096: 512 tiles = 3 waves + 116, whole tiles
+    monkeypatch.setenv("VITA_B200_GEMM_BN", "128")
+    _run(2048, 4352, 512, bias=True)             # 128-wide: 544 tiles = 4 waves + 16 -> pieces of 32 columns
 
 
 def test_gemm_tail_split_is_bit_identical_to_whole_tiles(monkeypatch):
@@ -74,7 +77,7 @@ def test_gemm_tail_split_is_bit_identical_to_whole_tiles(monkeypatch):
 
 
 def test_gemm_many_tiles_persistent():
-    # more tiles than SMs -> every CTA loops (smem ring phase wrap, both TMEM accumulator stages)
+    # more tiles than SMs -> every CTA loops (smem ring phase wrap across tiles)
     _run(1536, 8192, 512, bias=True)
 
 
@@ -189,26 +192,3 @@ def test_fused_router_permute_slot_layout_equals_align_gather_flow(T, H, I):
     ops.moe_combine(hb, ys, perm2, nxt, xb, 1e-5)
     torch.cuda.synchronize()
     assert torch.equal(ha, hb) and torch.equal(xa, xb)
-
-
-def test_moe_grouped_two_row_tiles_per_pass_keeps_the_bits(monkeypatch):
-    """MT = 2 (two 128-row tiles share every weight stage; gemm_sm100.cu) against one row tile per pass."""
-    from vita_b200 import ops
-    H, I, E = 1024, 2048, 8
-    counts = [130, 90, 256, 0, 257, 64, 127, 1]
-    rows = sum(counts)
-    offs = torch.tensor([0] + list(torch.tensor(counts).cumsum(0)), dtype=torch.int32).cuda()
-    x = to_dev(randn((rows, H), 1, 1.0))
-    w13, w2 = to_dev(randn((E, 2 * I, H), 2, 0.05)), to_dev(randn((E, H, I), 3, 0.05))
-    rw = torch.rand(rows, generator=torch.Generator().manual_seed(4)).cuda()
-    outs = []
-    for mt in ("1", "2"):
-        monkeypatch.setenv("VITA_B200_GEMM_MT", mt)
-        act = torch.full((rows, I), float("nan"), dtype=torch.bfloat16, device="cuda")
-        y = torch.full((rows, H), float("nan"), dtype=torch.bfloat16, device="cuda")
-        ops.moe_gate_up(x, w13, act, offs, rows)
-        ops.moe_down(act, w2, y, offs, rw, rows)
-        torch.cuda.synchronize()
-        outs.append((act, y))
-    assert torch.isfinite(outs[1][0].float()).all() and torch.isfinite(outs[1][1].float()).all()
-    assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1])

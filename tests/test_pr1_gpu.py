@@ -3,8 +3,7 @@
 
 (1) Against the fixture minted from the reference's own classes (oracle/make_golden_pr1.py mint --reference): every token
     id must equal the reference's -- no margin gating, no teacher forcing.  The weight scaling and the prompt seed that
-    make an fp32 trajectory reproducible in bf16 are described in oracle/pr1.py; profiles/r02_pr1_seed_search.json is
-    the search the seed came from.
+    make an fp32 trajectory reproducible in bf16 are described in oracle/pr1.py (the seed came from a search over prompts).
 (2) For other prompt seeds, against the fp32 oracle run on the same GPU with the routing aligned (tests/full_depth.py):
     every one of the 32 logits rows within tolerance and every id the oracle decides beyond that row's error equal.
     This form holds for ANY seed: a random-init MoE turns a rank-2 / rank-3 router near-tie on a prompt token into a

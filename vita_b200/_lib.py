@@ -86,7 +86,7 @@ def load() -> ctypes.CDLL:
     path = Path(os.environ.get("VITA_B200_LIB", LIB_PATH))
     if not path.exists():
         raise VitaB200Error(
-            f"{path} not found: build it with `python -m vita_b200.build` (nvcc, sm_100a). "
+            f"{path} not found: build it with `python -m vita_b200.build` (nvcc, sm_90a). "
             "There is no CPU or PyTorch fallback for the vita_b200 kernels.")
     lib = ctypes.CDLL(str(path))
     for name, (res, args) in SIGNATURES.items():

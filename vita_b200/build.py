@@ -1,4 +1,4 @@
-"""Builds vita_b200/lib/libvita_b200.so from vita_b200/csrc/*.cu with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds vita_b200/lib/libvita_b200.so from vita_b200/csrc/*.cu with nvcc for sm_90a (cross-compiles without a GPU).
 
 Used by ``__graft_entry__.build()`` and runnable directly: ``python -m vita_b200.build [--force]``.
 """
@@ -19,7 +19,7 @@ LIB = LIBDIR / "libvita_b200.so"
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -61,7 +61,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(lambda s: _compile_one(s, OBJDIR), srcs))
     tmp = LIB.with_suffix(".so.tmp")          # link aside, then rename: a reader never sees a half-written library
-    cmd = [NVCC, "-shared", "-o", str(tmp), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a",
+    cmd = [NVCC, "-shared", "-o", str(tmp), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a",
            "-lcudart"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:

@@ -468,7 +468,7 @@ extern "C" int vita_decode_attention(const void* q, const void* k_cache, const v
         resident_per_sm = n > 2 ? 2 : n;   // a chain neighbour may share the SM under programmatic launch
     }
     const bool tagged = option("attn_tagged") && (splits == 4 || splits == 8 || splits == 16) &&
-                        splits * n_kv_heads * B <= static_cast<long long>(resident_per_sm) * (num_sms() > 0 ? num_sms() : 148);
+                        splits * n_kv_heads * B <= static_cast<long long>(resident_per_sm) * (num_sms() > 0 ? num_sms() : 132);
     {
         static int carveout = -1;
         const int want = option("smem_carveout_max") ? cudaSharedmemCarveoutMaxShared : cudaSharedmemCarveoutDefault;

@@ -38,8 +38,7 @@ int make_tensor_map_bf16(CUtensorMap* out, const void* base, int rank, const uin
                          const uint32_t* box, bool swizzle128);
 
 // Programmatic dependent launch (PDL) for the decode chain: kernel N+1 may start (and prefetch weights) while kernel
-// N drains; it calls griddepcontrol.wait before touching anything N produced.  Opt-in with VITA_B200_PDL=1: on B200
-// it measured neutral with 1 CTA/SM footprints and 12% slower when the footprints allowed co-residency.
+// N drains; it calls griddepcontrol.wait before touching anything N produced.  Option "pdl" (VITA_B200_PDL).
 bool use_pdl();
 int option(const char* name);   // tunables table in api.cu (env default, vita_set_option override)
 

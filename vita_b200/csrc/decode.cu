@@ -1,4 +1,4 @@
-// Small kernels of the greedy-decode step (the linears are the tcgen05 GEMVs of decode_tc.cu):
+// Small kernels of the greedy-decode step (the linears are the wgmma GEMVs of decode_tc.cu):
 //   decode_embed   start of a step: consume the previous arg-max, log it, advance the cache length (saturating at the
 //                  KV capacity), bump the completion-counter serial, gather the embedding row
 //   decode_router  post-attention RMSNorm + router of one token per CTA (stand-alone form; the decode chain uses the

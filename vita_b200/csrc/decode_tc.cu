@@ -1,26 +1,27 @@
-// Decode-step linears on the 5th-gen tensor cores ("swap-AB" GEMV, stream-K):  y[rows] = W[rows, K] . x[K].
+// Decode-step linears on the tensor cores ("swap-AB" GEMV, stream-K):  y[rows] = W[rows, K] . x[K].
 //
-// The SIMT version of these kernels (decode.cu) moved every byte at full TMA rate but needed ~80 issue slots per
-// 32 bytes of weights for bf16->fp32 unpacking and FMAs, which capped it at ~65% of HBM bandwidth (ncu: 48% issue
-// utilisation at 60% DRAM throughput).  Here the weight tile is the *M* operand of tcgen05.mma (128 rows x 64 k,
+// A SIMT GEMV moves every byte at full TMA rate but needs ~80 issue slots per 32 bytes of weights for bf16->fp32
+// unpacking and FMAs.  Here the weight tile is the *M* operand of wgmma (128 rows x 64 k = two m64n16k16 row halves,
 // TMA-loaded with the 128B swizzle) and the activation vector is row 0 of a 16 x 64 *N* operand tile, so the CUDA
 // cores only run the per-row epilogue:
 //   warp 0  TMA producer: streams W tiles into an smem ring (starts before the PDL dependency resolves: weights
 //           never depend on the previous kernel, except for the expert ids which it waits for); once its last tile is
 //           issued it triggers the dependent launch, so the next kernel of the chain sets up and fills its own ring
 //           while this one drains and reduces;
-//   warp 1  MMA issuer: per ring stage, 4 x tcgen05.mma.kind::f16 (M=128, N=16, K=16) per part into TMEM;
-//   warp 2  TMEM allocator;
+//   warps 1-2  idle (they only take part in the wide router prologue);
 //   warp 3  x-tile writer: copies 128 B of the (bf16, smem-resident) activation vector into row 0 of the stage's
 //           N tile (rows 1..15 stay zero), fence.proxy.async, arrives on the stage barrier;
-//   warps 4-7  prologue (RMSNorm / router / residual prefetch) and epilogue: tcgen05.ld, fused per-row epilogue.
+//   warps 4-7  one warpgroup: prologue (RMSNorm / router / residual prefetch), then per ring stage 2 x 4 wgmma
+//           (M=64, N=16, K=16) per part into register accumulators, and the fused per-row epilogue (column 0 of the
+//           accumulator fragment goes through shared memory so that thread i owns row i of the block).
 // Work is cut stream-K style: the (row-block, k-block) units are split evenly and contiguously over the CTAs, so all
-// 148 SMs stream the same number of bytes whatever the matrix shape.  A row block whose K range spans several CTAs
+// SMs stream the same number of bytes whatever the matrix shape.  A row block whose K range spans several CTAs
 // is combined through per-contributor slots of 64-bit {partial, tag} words: no fence and no atomic, the CTA that ends
 // on the row block polls the others' words (collecting early arrivals while its own MMAs still run), adds them in
 // slot order (deterministic), clears the tags and runs the epilogue.
 #include "common.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace vita {
 
@@ -30,9 +31,6 @@ constexpr int TC_X_BYTES = TC_XN * 64 * 2;
 constexpr int TC_SLOTS = 8;               // max contributors per row block
 constexpr int TC_THREADS = 256;
 
-__device__ __forceinline__ void tmem_ld_32x32_x1(uint32_t taddr, uint32_t& r) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(taddr) : "memory");
-}
 __device__ __forceinline__ void epi_barrier() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 __device__ __forceinline__ unsigned long long ld_relaxed_u64(const unsigned long long* p) {
     unsigned long long v;
@@ -250,14 +248,12 @@ tc_gemv_kernel(const __grid_constant__ CUtensorMap tmW, const Op op, unsigned lo
     uint8_t* tail = reinterpret_cast<uint8_t*>(xs) + ((op.x_elems() * 2 + 127) / 128) * 128;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* acc_full = empty_bar + STAGES;
-    uint64_t* acc_empty = acc_full + 2;
-    uint64_t* x_ready = acc_empty + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(x_ready + 1);
-    float* scratch = reinterpret_cast<float*>(tmem_slot + 2);
+    uint64_t* x_ready = empty_bar + STAGES;
+    float* scratch = reinterpret_cast<float*>(x_ready + 1);
     float* prep = scratch + 64;
     float* pair = prep + 256;
-    int* misc = reinterpret_cast<int*>(pair + 128);
+    float* rows = pair + 128;          // [PARTS][128]: accumulator column 0, fragment layout -> one row per thread
+    int* misc = reinterpret_cast<int*>(rows + 2 * 128);
     TcSmem sm{xs, scratch, prep, misc, pair, x_ready};
 
     const int b = blockIdx.y;
@@ -278,26 +274,15 @@ tc_gemv_kernel(const __grid_constant__ CUtensorMap tmW, const Op op, unsigned lo
         tma_prefetch_desc(&tmW);
         for (int i = 0; i < STAGES; ++i) {
             mbar_init(&full_bar[i], 2);   // TMA producer (expect_tx) + x-tile writer
-            mbar_init(&empty_bar[i], 1);  // tcgen05.commit
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&acc_full[i], 1);
-            mbar_init(&acc_empty[i], 4);
+            mbar_init(&empty_bar[i], 4);  // the MMA warps, once their wgmma group has read the stage
         }
         mbar_init(x_ready, 1);
         fence_barrier_init();
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_slot, 64);
-        tmem_relinquish();
-    }
     // N-operand tiles: rows 1..15 stay zero for the whole kernel, row 0 is rewritten per stage
     for (int i = threadIdx.x; i < STAGES * STAGE_X / 16; i += TC_THREADS) reinterpret_cast<uint4*>(sX)[i] = make_uint4(0, 0, 0, 0);
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     if (threadIdx.x == 0) VITA_STAMP(2);
 
     // router-carrying op, wide form: every thread of the CTA takes part in the router dot products before the roles
@@ -366,43 +351,6 @@ tc_gemv_kernel(const __grid_constant__ CUtensorMap tmW, const Op op, unsigned lo
             }
             VITA_STAMP(6);
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ------------------------------------------------------------ MMA issuer
-            constexpr uint32_t idesc = umma_idesc_bf16(128, TC_XN);
-            const uint32_t sA_addr = smem_u32(sA), sX_addr = smem_u32(sX);
-            int stage = 0, acc = 0;
-            uint32_t phase = 0, acc_phase = 0;
-            long long u = u0;
-            if (flags & 4) chain_wait(chain);   // the activation vector derives from the predecessor: wait in hardware, not on full_bar
-            while (u < u1) {
-                const int rb = static_cast<int>(u / n_kb);
-                long long seg_end = static_cast<long long>(rb + 1) * n_kb;
-                if (seg_end > u1) seg_end = u1;
-                mbar_wait(&acc_empty[acc], acc_phase ^ 1, 23);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * 32;
-                for (long long v = u; v < seg_end; ++v) {
-                    mbar_wait(&full_bar[stage], phase, 24);
-                    tc_fence_after();
-                    if (v == u0) VITA_STAMP(5);
-#pragma unroll
-                    for (int p = 0; p < PARTS; ++p) {
-                        const uint64_t da = umma_desc_k_sw128(sA_addr + stage * STAGE_A + p * TC_A_BYTES);
-                        const uint64_t dx = umma_desc_k_sw128(sX_addr + stage * STAGE_X + (XPARTS > 1 ? p : 0) * TC_X_BYTES);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            tc_mma_bf16(d_tmem + p * TC_XN, da + 2 * k, dx + 2 * k, idesc, (v > u || k > 0) ? 1u : 0u);
-                    }
-                    tc_commit(&empty_bar[stage]);
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-                tc_commit(&acc_full[acc]);
-                acc ^= 1;
-                if (acc == 0) acc_phase ^= 1;
-                u = seg_end;
-            }
-        }
     } else if (warp == 3) {
         // ---------------------------------------------------------------- x-tile writer
         // per stage: copy 128 B of the activation vector into row 0 of the N tile
@@ -457,8 +405,10 @@ tc_gemv_kernel(const __grid_constant__ CUtensorMap tmW, const Op op, unsigned lo
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp >= 4) {
-        // ---------------------------------------------------------------- prologue + epilogue (128 threads)
+    }
+    if (warp < 4) return;   // the MMA warpgroup continues at the top level: wgmma inside a role branch is serialised by ptxas
+    {
+        // ---------------------------------------------------------------- prologue + MMA + epilogue (128 threads)
         if (!wide) op.pre_wait(b, sm, (flags & 1) != 0);   // constants only: L2 prefetch ahead of the dependency wait
         if (threadIdx.x == 128) chain_wait(chain);   // activations come from the previous kernel
         epi_barrier();
@@ -470,10 +420,11 @@ tc_gemv_kernel(const __grid_constant__ CUtensorMap tmW, const Op op, unsigned lo
 
         const int quad = warp - 4;
         const int row = quad * 32 + lane;
+        const uint32_t sA_addr = smem_u32(sA), sX_addr = smem_u32(sX);
+        int stage = 0;
+        uint32_t phase = 0;
         TcFinish st{-INFINITY, 0x7fffffff};
         unsigned long long* my_scratch = g_scratch + static_cast<long long>(b) * n_rb * TC_SLOTS * PARTS * 128;
-        int acc = 0;
-        uint32_t acc_phase = 0;
         long long u = u0;
         while (u < u1) {
             const int rb = static_cast<int>(u / n_kb);
@@ -513,22 +464,61 @@ tc_gemv_kernel(const __grid_constant__ CUtensorMap tmW, const Op op, unsigned lo
                     }
                 }
             }
-            mbar_wait(&acc_full[acc], acc_phase, 27);
-            tc_fence_after();
+            // ---- the segment's MMAs: d[p][mh] is rows [64 mh, 64 mh + 64) of part p; one wgmma group in flight, a
+            // ring stage goes back to the producer and the x-tile writer once the group that read it has completed
+            float d[PARTS][2][TC_XN / 2];
+            int prev = -1;
+            for (long long w = u; w < seg_end; ++w) {
+                mbar_wait(&full_bar[stage], phase, 24);
+                if (threadIdx.x == 128 && w == u0) VITA_STAMP(5);
+#pragma unroll
+                for (int p = 0; p < PARTS; ++p) { wgmma_acc_fence(d[p][0]); wgmma_acc_fence(d[p][1]); }
+                wgmma_fence();
+#pragma unroll
+                for (int p = 0; p < PARTS; ++p) {
+                    const uint64_t dx = wgmma_desc_k_sw128(sX_addr + stage * STAGE_X + (XPARTS > 1 ? p : 0) * TC_X_BYTES);
+#pragma unroll
+                    for (int mh = 0; mh < 2; ++mh) {
+                        const uint64_t da = wgmma_desc_k_sw128(sA_addr + stage * STAGE_A + p * TC_A_BYTES + mh * (64 * 128));
+#pragma unroll
+                        for (int k = 0; k < 4; ++k)
+                            wgmma_ss<TC_XN>(d[p][mh], da + 2 * k, dx + 2 * k, (w > u || k > 0) ? 1 : 0);
+                    }
+                }
+                wgmma_commit();
+#pragma unroll
+                for (int p = 0; p < PARTS; ++p) { wgmma_acc_fence(d[p][0]); wgmma_acc_fence(d[p][1]); }
+                wgmma_wait<1>();   // unconditional (a no-op for the first stage): warpgroup-wide, must not sit in a branch
+                if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+                prev = stage;
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+#pragma unroll
+            for (int p = 0; p < PARTS; ++p) { wgmma_acc_fence(d[p][0]); wgmma_acc_fence(d[p][1]); }
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
             if (threadIdx.x == 128 && seg_end == u1) VITA_STAMP(7);
+            // column 0 of the fragment (lanes 0, 4, ..: rows 16 quad + lane / 4 and + 8 of each half) -> thread-per-row.
+            // (every lane reads its accumulators; only the store is conditional)
+            float c0[PARTS][2][2];
+#pragma unroll
+            for (int p = 0; p < PARTS; ++p)
+#pragma unroll
+                for (int mh = 0; mh < 2; ++mh) { c0[p][mh][0] = d[p][mh][0]; c0[p][mh][1] = d[p][mh][2]; }
+            if ((lane & 3) == 0) {
+#pragma unroll
+                for (int p = 0; p < PARTS; ++p)
+#pragma unroll
+                    for (int mh = 0; mh < 2; ++mh) {
+                        rows[p * 128 + mh * 64 + quad * 16 + (lane >> 2)] = c0[p][mh][0];
+                        rows[p * 128 + mh * 64 + quad * 16 + (lane >> 2) + 8] = c0[p][mh][1];
+                    }
+            }
+            epi_barrier();
             float v[PARTS];
 #pragma unroll
-            for (int p = 0; p < PARTS; ++p) {
-                uint32_t r;
-                tmem_ld_32x32_x1(tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + acc * 32 + p * TC_XN, r);
-                v[p] = __uint_as_float(r);
-            }
-            tmem_ld_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[acc]);
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1;
+            for (int p = 0; p < PARTS; ++p) v[p] = rows[p * 128 + row];
+            epi_barrier();
 
             bool do_finish = true;
             if (partial && slot != 0) {
@@ -574,12 +564,6 @@ tc_gemv_kernel(const __grid_constant__ CUtensorMap tmW, const Op op, unsigned lo
         if (threadIdx.x == 128) VITA_STAMP(8);
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 64);
-    }
 }
 
 // ------------------------------------------------------------------------------------------------ ops
@@ -774,7 +758,7 @@ struct TcGateUpOp {
 };
 
 struct TcDownOp {
-    static constexpr int kMaxRegs = 96;
+    static constexpr int kMaxRegs = 112;
     static constexpr int kId = 5;
     static constexpr bool kXFromGlobal = true;
     static constexpr bool kBulkX = false;
@@ -900,8 +884,8 @@ static int launch_tc(const Op& op, const void* W, long long w_rows, int K, int n
     int rc = make_tensor_map_bf16(&tm, W, 2, dims, strides, box, true);
     if (rc) return rc;
     const int smem_bytes = Op::kStages * (Op::kParts * TC_A_BYTES + Op::kXParts * TC_X_BYTES) +
-                           ((x_elems * 2 + 127) / 128) * 128 + (2 * Op::kStages + 5) * 8 + 8 +
-                           (64 + 256 + 128 + 8) * 4 + 1024 + 128;
+                           ((x_elems * 2 + 127) / 128) * 128 + (2 * Op::kStages + 1) * 8 +
+                           (64 + 256 + 128 + 256 + 8) * 4 + 1024 + 128;
     auto kern = tc_gemv_kernel<Op>;
     static int configured = 0;
     if (smem_bytes > configured) {

@@ -1,5 +1,5 @@
 // HBM-bound row kernels of the omni forward path: norms, embedding gather / splice scatter, RoPE + paged-KV write,
-// MoE router / align / gather / combine, and the im2col / layout kernels that feed the tcgen05 GEMM for the
+// MoE router / align / gather / combine, and the im2col / layout kernels that feed the wgmma GEMM for the
 // convolutional front-ends.  All of them are one-pass, 16-byte vectorised, fp32 math, bf16 storage.
 #include "common.h"
 #include "ptx.cuh"
@@ -1023,7 +1023,7 @@ extern "C" int vita_ep_push(void* const* peer_base, const int64_t* offsets, cons
     r.n = static_cast<int>(n_ranges);
     if (total == 0 || n_ranks == 1) return VITA_OK;
     long long blocks = (total / 16 + 255) / 256 + 1;
-    const int cap = 2 * (num_sms() > 0 ? num_sms() : 148);
+    const int cap = 2 * (num_sms() > 0 ? num_sms() : 132);
     if (blocks > cap) blocks = cap;
     ep_push_kernel<<<static_cast<unsigned>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         reinterpret_cast<uint8_t* const*>(peer_base), r, (int)n_ranks, (int)my_rank);

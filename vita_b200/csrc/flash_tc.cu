@@ -1,16 +1,14 @@
-// FlashAttention forward for sm_100a on the 5th-generation tensor cores:  O = softmax(Q K^T * scale [masks]) V.
+// FlashAttention forward for sm_90a on wgmma:  O = softmax(Q K^T * scale [masks]) V.
 //
-// One CTA owns NQ (1 or 2) query tiles of 128 rows and walks the keys in tiles of 128:
-//   warp  4*NQ     : TMA producer  (cp.async.bulk.tensor 4-D boxes, 128B swizzle: Q once, K / V through mbarrier rings)
-//   warp  4*NQ + 1 : MMA issuer    (one thread; S_t = Q_t K_j^T as tcgen05.mma SS, O_t += P_t V_j as tcgen05.mma TS with
-//                                   the probabilities read from tensor memory and V as an MN-major shared operand)
-//   warps 4t..4t+3 : softmax group of query tile t (thread = query row): tcgen05.ld S -> running max / exp2 / sum ->
-//                    bf16 P written back over S with tcgen05.st; rescales the O accumulator in TMEM only when the
-//                    running max moved by more than 2^8 (the final 1/l normalisation absorbs the stale reference)
-// TMEM: S_t (128 fp32 columns, P_t aliases its first 64) and O_t (DV columns) per query tile.  With two query tiles
-// the tensor core works on one tile (PV_t(j), then S_t(j+1), issued back to back) while the other tile's softmax
-// group runs.  tcgen05.commit after S_t(j+1) also covers PV_t(j), so "S_t full" tells the softmax group that O_t is
-// complete through tile j: no separate accumulator barrier is needed for the rescale.
+// One CTA owns a query tile of 128 rows and walks the keys in tiles of 128 (384 threads):
+//   warpgroup 0    : TMA producer (one thread; cp.async.bulk.tensor 4-D boxes, 128B swizzle: Q once, K / V through
+//                    mbarrier rings); gives its registers to the consumers with setmaxnreg
+//   warpgroups 1-2 : consumers, 64 query rows each.  S = Q K_j^T as wgmma m64n128k16 with both operands from shared
+//                    memory; running max / exp2 / sum on the accumulator fragment (a row lives in the four lanes of a
+//                    quad); the bf16 probabilities stay in registers as the A operand of O += P V_j (wgmma with V as
+//                    an MN-major shared operand).  The O accumulator is rescaled only when the running max moved by
+//                    more than 2^8 (the final 1/l normalisation absorbs the stale reference).
+// Inside a warpgroup MMA and softmax alternate; the two warpgroups are independent and can overlap each other.
 //
 // Serves the three prefill-shaped attentions of the path (reference call sites):
 //   Mixtral causal GQA 128/128  transformers sdpa / eager attention (modeling_mixtral.py:269-292)
@@ -18,6 +16,7 @@
 //   Whale rel-pos 128/64        attention.py:391-415, both score terms as one contraction over [k | p], key padding
 #include "common.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace vita {
 
@@ -31,37 +30,34 @@ struct FaParams {
     int q_pos0;                   // causal: key position of query row 0 (rows of a sequence shard start later)
     float scale_log2;             // softmax scale * log2(e)
     int n_qblk;                   // number of 128-row query blocks
-    int pair_heads;               // NQ == 2: 1 = tiles are heads (2y, 2y+1) at the same rows, 0 = rows (2x, 2x+1)
-    uint32_t v_lbo, v_sbo;        // MN-major descriptor strides of the V tile (bytes)
     int poly_chunks;              // of the 4 column chunks of a tile, how many take exp2 on the FMA pipe (MUFU relief)
 };
 
-constexpr int FA_BM = 128;   // query rows per tile (UMMA M, TMEM lanes)
+constexpr int FA_BM = 128;   // query rows per tile (64 per consumer warpgroup)
 constexpr int FA_BN = 128;   // keys per tile
 
-template <int DQK, int DV, int NQ>
+template <int DQK, int DV>
 struct FaCfg {
     static constexpr int STAGES = (DQK == 128 && DV == 128) ? 2 : (DQK == 128 ? 3 : 4);
     static constexpr int Q_BYTES = FA_BM * DQK * 2;
     static constexpr int K_BYTES = FA_BN * DQK * 2;
     static constexpr int V_BYTES = FA_BN * DV * 2;
-    static constexpr int THREADS = 128 * NQ + 128;   // softmax groups + one control warpgroup (TMA, MMA, 2 idle warps)
-    static constexpr int TMEM_COLS = NQ * (128 + DV) <= 256 ? 256 : 512;
-    static constexpr int SMEM = NQ * Q_BYTES + STAGES * (K_BYTES + V_BYTES) + 1024 /*align*/ + 256 /*barriers*/;
+    static constexpr int THREADS = 384;
+    static constexpr int SMEM = Q_BYTES + STAGES * (K_BYTES + V_BYTES) + 1024 /*align*/ + 256 /*barriers*/;
 };
 
-template <int DQK, int DV, int NQ, int POLY>
-__global__ void __launch_bounds__(FaCfg<DQK, DV, NQ>::THREADS, 1)
+template <int DQK, int DV, int POLY>
+__global__ void __launch_bounds__(FaCfg<DQK, DV>::THREADS, 1)
 flash_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FaParams p) {
-    using Cfg = FaCfg<DQK, DV, NQ>;
+    using Cfg = FaCfg<DQK, DV>;
     constexpr int ST = Cfg::STAGES;
     constexpr int HALF = FA_BM * 128;   // bytes of one 64-column block of a 128-row tile ([128 rows][128 B])
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sQ = smem;
-    uint8_t* sK = sQ + NQ * Cfg::Q_BYTES;
+    uint8_t* sK = sQ + Cfg::Q_BYTES;
     uint8_t* sV = sK + ST * Cfg::K_BYTES;
     uint64_t* bars = reinterpret_cast<uint64_t*>(sV + ST * Cfg::V_BYTES);
     uint64_t* q_full = bars;
@@ -69,46 +65,29 @@ flash_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     uint64_t* k_empty = k_full + ST;
     uint64_t* v_full = k_empty + ST;
     uint64_t* v_empty = v_full + ST;
-    uint64_t* s_full = v_empty + ST;       // [NQ] S_t(j) is in TMEM (and O_t is complete through tile j-1)
-    uint64_t* p_ready = s_full + NQ;       // [NQ] P_t(j) is in TMEM, O_t rescaled
-    uint64_t* o_final = p_ready + NQ;      // [NQ]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_final + NQ);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int b = blockIdx.z;
 
-    // ---- which query tiles does this CTA own?  (long causal rows first)
+    // long causal rows first
     const int bx = p.causal ? static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x) : static_cast<int>(blockIdx.x);
-    int head[NQ], q0[NQ];
-    if constexpr (NQ == 1) {
-        head[0] = blockIdx.y;
-        q0[0] = bx * FA_BM;
-    } else {
-        if (p.pair_heads) {
-            head[0] = 2 * blockIdx.y; head[1] = head[0] + 1;
-            q0[0] = q0[1] = bx * FA_BM;
-        } else {
-            head[0] = head[1] = blockIdx.y;
-            q0[0] = 2 * bx * FA_BM; q0[1] = q0[0] + FA_BM;
-        }
-    }
-    const int kvh = head[0] / p.group;
+    const int head = blockIdx.y;
+    const int q0 = bx * FA_BM;
+    const int kvh = head / p.group;
     int kv_len = p.kv_lens ? p.kv_lens[b] : p.Skv;
     if (kv_len > p.Skv) kv_len = p.Skv;
     if (kv_len < 0) kv_len = 0;
     int n_tiles = (kv_len + FA_BN - 1) / FA_BN;
     if (p.causal) {
-        const int lim = (p.q_pos0 + q0[NQ - 1] + FA_BM + FA_BN - 1) / FA_BN;   // keys <= last row of the last tile
+        const int lim = (p.q_pos0 + q0 + FA_BM + FA_BN - 1) / FA_BN;   // keys <= last row of the tile
         if (n_tiles > lim) n_tiles = lim;
     }
 
-    if (n_tiles == 0) {   // no keys at all: zeros (uniform over the CTA, nothing allocated yet)
-        if (warp < 4 * NQ) {
-            const bool second = (NQ == 2 && (warp >> 2) == 1);
-            const int row = (second ? q0[NQ - 1] : q0[0]) + (warp & 3) * 32 + lane;
+    if (n_tiles == 0) {   // no keys at all: zeros (uniform over the CTA)
+        if (threadIdx.x >= 128 && threadIdx.x < 128 + FA_BM) {
+            const int row = q0 + static_cast<int>(threadIdx.x) - 128;
             if (row < p.Sq) {
-                uint4* orow = reinterpret_cast<uint4*>(p.o + b * p.o_bs + static_cast<long long>(row) * p.o_ts +
-                                                       (second ? head[NQ - 1] : head[0]) * p.o_hs);
+                uint4* orow = reinterpret_cast<uint4*>(p.o + b * p.o_bs + static_cast<long long>(row) * p.o_ts + head * p.o_hs);
                 for (int i = 0; i < DV / 8; ++i) orow[i] = make_uint4(0, 0, 0, 0);
             }
         }
@@ -122,41 +101,22 @@ flash_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         mbar_init(q_full, 1);
         for (int i = 0; i < ST; ++i) {
             mbar_init(&k_full[i], 1);
-            mbar_init(&k_empty[i], 1);
+            mbar_init(&k_empty[i], 8);   // one arrival per consumer warp
             mbar_init(&v_full[i], 1);
-            mbar_init(&v_empty[i], 1);
-        }
-        for (int t = 0; t < NQ; ++t) {
-            mbar_init(&s_full[t], 1);
-            mbar_init(&p_ready[t], 128);
-            mbar_init(&o_final[t], 1);
+            mbar_init(&v_empty[i], 8);
         }
         fence_barrier_init();
     }
-    if (warp == 4 * NQ + 1) {
-        tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    // TMEM columns: S_t at t*128 (P_t aliases the first 64 of them), O_t at NQ*128 + t*DV
 
-    // Two query tiles: 384 threads leave 168 registers per thread, short of the 128 scores a softmax thread keeps
-    // live; the control warpgroup hands its registers to the softmax groups.  The pool is what the CTA got at launch
-    // (384 x 168): 128 x (168 - 72) released = 2 x 128 x (216 - 168) claimed, exactly.
-    if (warp >= 4 * NQ) {
-        if constexpr (NQ == 2) asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
-      if (warp == 4 * NQ) {
+    if (warp < 4) {
         // ------------------------------------------------------------------------------------ TMA producer
-        if (lane == 0) {
-            mbar_arrive_expect_tx(q_full, NQ * Cfg::Q_BYTES);
+        // 384 x 168 registers at launch = 128 x 40 + 256 x 232
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (threadIdx.x == 0) {
+            mbar_arrive_expect_tx(q_full, Cfg::Q_BYTES);
 #pragma unroll
-            for (int t = 0; t < NQ; ++t)
-#pragma unroll
-                for (int c = 0; c < DQK / 64; ++c)
-                    tma_load_4d(sQ + t * Cfg::Q_BYTES + c * HALF, &tmQ, q_full, c * 64, q0[t], head[t], b);
+            for (int c = 0; c < DQK / 64; ++c) tma_load_4d(sQ + c * HALF, &tmQ, q_full, c * 64, q0, head, b);
             int stage = 0;
             uint32_t phase = 0;
             for (int j = 0; j < n_tiles; ++j) {
@@ -173,177 +133,133 @@ flash_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
                 if (++stage == ST) { stage = 0; phase ^= 1; }
             }
         }
-      } else if (warp == 4 * NQ + 1) {
-        // ------------------------------------------------------------------------------------ MMA issuer
-        if (lane == 0) {
-            constexpr uint32_t idesc_s = umma_idesc_bf16(FA_BM, FA_BN);                 // Q, K both K-major
-            constexpr uint32_t idesc_o = umma_idesc_bf16(FA_BM, DV) | (1u << 16);       // V is MN-major
-            const uint32_t sQ_a = smem_u32(sQ), sK_a = smem_u32(sK), sV_a = smem_u32(sV);
-            auto issue_s = [&](int t, int stage) {
-                const uint32_t qa = sQ_a + t * Cfg::Q_BYTES, ka = sK_a + stage * Cfg::K_BYTES;
-#pragma unroll
-                for (int k = 0; k < DQK / 16; ++k) {
-                    const uint32_t off = (k >> 2) * HALF + (k & 3) * 32;   // 64-column block, then 32 B per 16 elements
-                    tc_mma_bf16(tmem_base + t * 128, umma_desc_k_sw128(qa + off), umma_desc_k_sw128(ka + off), idesc_s,
-                                k != 0 ? 1u : 0u);
-                }
-            };
-            auto issue_pv = [&](int t, int stage, bool acc) {
-                const uint32_t va = sV_a + stage * Cfg::V_BYTES;
-#pragma unroll
-                for (int k = 0; k < FA_BN / 16; ++k)   // 16 keys per instruction: 16 rows of 128 B, 8 packed P columns
-                    tc_mma_bf16_ts(tmem_base + NQ * 128 + t * DV, tmem_base + t * 128 + k * 8,
-                                   umma_desc_mn_sw128(va + k * 2048, p.v_lbo, p.v_sbo), idesc_o,
-                                   (acc || k != 0) ? 1u : 0u);
-            };
-            mbar_wait(q_full, 0, 20);
-            mbar_wait(&k_full[0], 0, 21);
-            tc_fence_after();
-#pragma unroll
-            for (int t = 0; t < NQ; ++t) {
-                issue_s(t, 0);
-                tc_commit(&s_full[t]);
-            }
-            tc_commit(&k_empty[0]);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int j = 0; j < n_tiles; ++j) {
-                int nstage = stage + 1;
-                uint32_t nphase = phase;
-                if (nstage == ST) { nstage = 0; nphase ^= 1; }
-                mbar_wait(&v_full[stage], phase, 22);
-#pragma unroll
-                for (int t = 0; t < NQ; ++t) {
-                    mbar_wait(&p_ready[t], j & 1, 23);
-                    tc_fence_after();
-                    issue_pv(t, stage, j > 0);
-                    if (t == NQ - 1) tc_commit(&v_empty[stage]);
-                    if (j + 1 < n_tiles) {
-                        if (t == 0) {
-                            mbar_wait(&k_full[nstage], nphase, 24);
-                            tc_fence_after();
-                        }
-                        issue_s(t, nstage);       // overwrites S_t / P_t: ordered after PV_t(j) by issue order
-                        tc_commit(&s_full[t]);
-                        if (t == NQ - 1) tc_commit(&k_empty[nstage]);
-                    } else {
-                        tc_commit(&o_final[t]);
-                    }
-                }
-                stage = nstage;
-                phase = nphase;
-            }
-        }
-      }
-    } else {
-        // ------------------------------------------------------------------------------------ softmax groups
-        if constexpr (NQ == 2) asm volatile("setmaxnreg.inc.sync.aligned.u32 216;");
-        const int t = warp >> 2, quad = warp & 3;
-        const int my_q0 = (NQ == 2 && t == 1) ? q0[NQ - 1] : q0[0];
-        const int my_head = (NQ == 2 && t == 1) ? head[NQ - 1] : head[0];
-        const int row = my_q0 + quad * 32 + lane;             // global query row of this thread
-        const uint32_t lane_base = static_cast<uint32_t>(quad * 32) << 16;
-        const uint32_t tS = tmem_base + lane_base + t * 128;
-        const uint32_t tO = tmem_base + lane_base + NQ * 128 + t * DV;
-        float m_ref = -INFINITY, l = 0.0f;
-        for (int j = 0; j < n_tiles; ++j) {
-            mbar_wait(&s_full[t], j & 1, 30);
-            tc_fence_after();
-            uint32_t v[128];
-#pragma unroll
-            for (int c = 0; c < 4; ++c) tmem_ld_32x32(tS + c * 32, *reinterpret_cast<uint32_t(*)[32]>(&v[c * 32]));
-            tmem_ld_wait();
-            const int col0 = j * FA_BN;
-            const bool boundary = (col0 + FA_BN > kv_len) || (p.causal && col0 + FA_BN - 1 > p.q_pos0 + my_q0);   // warp-uniform
-            if (boundary) {
-                const int lim = p.causal ? min(kv_len, p.q_pos0 + row + 1) : kv_len;   // columns >= lim are masked
-#pragma unroll
-                for (int i = 0; i < 128; ++i)
-                    if (col0 + i >= lim) v[i] = 0xff800000u;   // -inf
-            }
-            float mx = -INFINITY;
-#pragma unroll
-            for (int i = 0; i < 128; i += 2) mx = fmax3(mx, __uint_as_float(v[i]), __uint_as_float(v[i + 1]));
-            const float m_new = fmaxf(m_ref, mx * p.scale_log2);
-            const bool grow = m_new > m_ref + 8.0f;
-            if (__any_sync(0xffffffffu, grow)) {
-                // move the reference of the rows that need it (the decision is per row, so a row's result does not
-                // depend on its warp neighbours): rescale the row sum and the accumulator
-                const float alpha = grow ? ex2_approx(m_ref - m_new) : 1.0f;
-                l *= alpha;
-                if (grow) m_ref = m_new;
-                if (j > 0) {
-#pragma unroll
-                    for (int c = 0; c < DV / 32; ++c) {
-                        uint32_t o[32];
-                        tmem_ld_32x32(tO + c * 32, o);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-                        tmem_st_32x32(tO + c * 32, o);
-                    }
-                }
-            }
-            const float m_use = (m_ref == -INFINITY) ? 0.0f : m_ref;
-            float2 sum2 = make_float2(0.0f, 0.0f);
-            const float2 sc2 = make_float2(p.scale_log2, p.scale_log2), nm2 = make_float2(-m_use, -m_use);
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {   // 32 scores -> 16 packed bf16 pairs -> P columns [16c, 16c + 16)
-                uint32_t pk[16];
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const float2 x = ffma2(make_float2(__uint_as_float(v[c * 32 + 2 * i]), __uint_as_float(v[c * 32 + 2 * i + 1])),
-                                           sc2, nm2);
-                    const float2 a = (c < POLY) ? ex2_poly2(x) : make_float2(ex2_approx(x.x), ex2_approx(x.y));
-                    sum2 = fadd2(sum2, a);
-                    pk[i] = pack_bf16(a.x, a.y);
-                }
-                tmem_st_32x16(tS + c * 16, pk);
-            }
-            l += sum2.x + sum2.y;
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(&p_ready[t]);
-        }
-        // ---- epilogue: O / l -> bf16 -> global
-        mbar_wait(&o_final[t], 0, 31);
-        tc_fence_after();
-        const float inv = l > 0.0f ? 1.0f / l : 0.0f;
-        __nv_bfloat16* orow = p.o + b * p.o_bs + static_cast<long long>(row) * p.o_ts + my_head * p.o_hs;
-#pragma unroll
-        for (int c = 0; c < DV / 32; ++c) {
-            uint32_t o[32];
-            tmem_ld_32x32(tO + c * 32, o);
-            tmem_ld_wait();
-            if (row < p.Sq) {
-                uint4* dst = reinterpret_cast<uint4*>(orow + c * 32);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    uint4 w;
-                    w.x = pack_bf16(__uint_as_float(o[q * 8 + 0]) * inv, __uint_as_float(o[q * 8 + 1]) * inv);
-                    w.y = pack_bf16(__uint_as_float(o[q * 8 + 2]) * inv, __uint_as_float(o[q * 8 + 3]) * inv);
-                    w.z = pack_bf16(__uint_as_float(o[q * 8 + 4]) * inv, __uint_as_float(o[q * 8 + 5]) * inv);
-                    w.w = pack_bf16(__uint_as_float(o[q * 8 + 6]) * inv, __uint_as_float(o[q * 8 + 7]) * inv);
-                    dst[q] = w;
-                }
-            }
-        }
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4 * NQ + 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+    // ------------------------------------------------------------------------------------ consumers
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cw = (warp >> 2) - 1;                    // rows [64 cw, 64 cw + 64) of the query tile
+    const int qr = lane >> 2, qc = lane & 3;
+    const int wg_q0 = q0 + cw * 64;
+    int row[2];
+    row[0] = wg_q0 + (warp & 3) * 16 + qr;
+    row[1] = row[0] + 8;
+    const uint32_t sQ_a = smem_u32(sQ) + cw * (64 * 128), sK_a = smem_u32(sK), sV_a = smem_u32(sV);
+    float o[DV / 2];
+#pragma unroll
+    for (int i = 0; i < DV / 2; ++i) o[i] = 0.0f;
+    float m_ref[2] = {-INFINITY, -INFINITY}, l[2] = {0.0f, 0.0f};   // l: this thread's share of the row sum
+    int stage = 0;
+    uint32_t phase = 0;
+    mbar_wait(q_full, 0, 20);
+    for (int j = 0; j < n_tiles; ++j) {
+        // ---- S = Q K_j^T
+        float s[FA_BN / 2];
+        mbar_wait(&k_full[stage], phase, 21);
+        wgmma_acc_fence(s);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < DQK / 16; ++k) {
+            const uint32_t off = (k >> 2) * HALF + (k & 3) * 32;   // 64-column block, then 32 B per 16 elements
+            wgmma_ss<FA_BN>(s, wgmma_desc_k_sw128(sQ_a + off), wgmma_desc_k_sw128(sK_a + stage * Cfg::K_BYTES + off),
+                            k != 0 ? 1 : 0);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_acc_fence(s);
+        if (lane == 0) mbar_arrive(&k_empty[stage]);
+
+        // ---- softmax on the fragment: s[4 jb + 2 h + e] is row[h], key col0 + 8 jb + 2 qc + e
+        const int col0 = j * FA_BN;
+        const bool boundary = (col0 + FA_BN > kv_len) || (p.causal && col0 + FA_BN - 1 > p.q_pos0 + wg_q0);   // warp-uniform
+        if (boundary) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int lim = p.causal ? min(kv_len, p.q_pos0 + row[h] + 1) : kv_len;   // columns >= lim are masked
+#pragma unroll
+                for (int jb = 0; jb < FA_BN / 8; ++jb)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e)
+                        if (col0 + jb * 8 + 2 * qc + e >= lim) s[4 * jb + 2 * h + e] = -INFINITY;
+            }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float mx = -INFINITY;
+#pragma unroll
+            for (int jb = 0; jb < FA_BN / 8; ++jb) mx = fmaxf(mx, fmaxf(s[4 * jb + 2 * h], s[4 * jb + 2 * h + 1]));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            const float m_new = fmaxf(m_ref[h], mx * p.scale_log2);
+            if (m_new > m_ref[h] + 8.0f) {
+                // move the reference of this row (the decision is per row, identical in its four lanes): rescale the
+                // row sum and the accumulator
+                const float alpha = ex2_approx(m_ref[h] - m_new);
+                l[h] *= alpha;
+                m_ref[h] = m_new;
+                if (j > 0) {
+#pragma unroll
+                    for (int jb = 0; jb < DV / 8; ++jb) {
+                        o[4 * jb + 2 * h] *= alpha;
+                        o[4 * jb + 2 * h + 1] *= alpha;
+                    }
+                }
+            }
+            const float m_use = (m_ref[h] == -INFINITY) ? 0.0f : m_ref[h];
+            float sum = 0.0f;
+#pragma unroll
+            for (int jb = 0; jb < FA_BN / 8; ++jb)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const float x = fmaf(s[4 * jb + 2 * h + e], p.scale_log2, -m_use);
+                    const float a = ((jb >> 2) < POLY) ? ex2_poly(x) : ex2_approx(x);
+                    sum += a;
+                    s[4 * jb + 2 * h + e] = a;
+                }
+            l[h] += sum;
+        }
+
+        // ---- O += P V_j: 16 keys per instruction, P from registers, V rows of 128 B as an MN-major operand (64-column
+        // blocks FA_BN * 128 B apart, 8-key groups 1024 B apart)
+        mbar_wait(&v_full[stage], phase, 22);
+        wgmma_acc_fence(o);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < FA_BN / 16; ++kk) {
+            const uint32_t a[4] = {pack_bf16(s[8 * kk + 0], s[8 * kk + 1]), pack_bf16(s[8 * kk + 2], s[8 * kk + 3]),
+                                   pack_bf16(s[8 * kk + 4], s[8 * kk + 5]), pack_bf16(s[8 * kk + 6], s[8 * kk + 7])};
+            wgmma_rs_bt<DV>(o, a, wgmma_desc_mn_sw128(sV_a + stage * Cfg::V_BYTES + kk * 2048, FA_BN * 128, 1024),
+                            (j > 0 || kk > 0) ? 1 : 0);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_acc_fence(o);
+        if (lane == 0) mbar_arrive(&v_empty[stage]);
+        if (++stage == ST) { stage = 0; phase ^= 1; }
+    }
+
+    // ---- epilogue: O / l -> bf16 -> global
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float lt = l[h];
+        lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+        lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+        const float inv = lt > 0.0f ? 1.0f / lt : 0.0f;
+        if (row[h] < p.Sq) {
+            __nv_bfloat16* orow = p.o + b * p.o_bs + static_cast<long long>(row[h]) * p.o_ts + head * p.o_hs;
+#pragma unroll
+            for (int jb = 0; jb < DV / 8; ++jb)
+                *reinterpret_cast<uint32_t*>(orow + jb * 8 + 2 * qc) = pack_bf16(o[4 * jb + 2 * h] * inv, o[4 * jb + 2 * h + 1] * inv);
+        }
     }
 }
 
-template <int DQK, int DV, int NQ, int POLY>
+template <int DQK, int DV, int POLY>
 static int launch_flash_tc_p(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const FaParams& p,
                              dim3 grid, cudaStream_t st) {
-    using Cfg = FaCfg<DQK, DV, NQ>;
+    using Cfg = FaCfg<DQK, DV>;
     static bool configured = false;
-    auto kern = flash_tc_kernel<DQK, DV, NQ, POLY>;
+    auto kern = flash_tc_kernel<DQK, DV, POLY>;
     if (!configured) {
         int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM),
                             "cudaFuncSetAttribute(flash_tc smem)");
@@ -355,11 +271,11 @@ static int launch_flash_tc_p(const CUtensorMap& tmQ, const CUtensorMap& tmK, con
 }
 
 // POLY = column chunks (of 4 per key tile) whose exp2 runs as a polynomial on the FMA pipe (option "fa_poly")
-template <int DQK, int DV, int NQ>
+template <int DQK, int DV>
 static int launch_flash_tc(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const FaParams& p,
                            dim3 grid, cudaStream_t st) {
-    if (p.poly_chunks >= 1) return launch_flash_tc_p<DQK, DV, NQ, 1>(tmQ, tmK, tmV, p, grid, st);
-    return launch_flash_tc_p<DQK, DV, NQ, 0>(tmQ, tmK, tmV, p, grid, st);
+    if (p.poly_chunks >= 1) return launch_flash_tc_p<DQK, DV, 1>(tmQ, tmK, tmV, p, grid, st);
+    return launch_flash_tc_p<DQK, DV, 0>(tmQ, tmK, tmV, p, grid, st);
 }
 
 // 4-D view (D, tokens, heads, batch) of a strided activation; box = 64 columns x 128 tokens, 128B swizzle
@@ -387,24 +303,9 @@ static int flash_tc_dispatch(const void* q, const void* k, const void* v, const 
     rc = make_qkv_map(&tmV, v, DV, p.Skv, Hkv, B, vs[1], vs[2], vs[0]);
     if (rc) return rc;
     p.n_qblk = (p.Sq + FA_BM - 1) / FA_BM;
-    p.v_lbo = option("fa_v_lbo") ? static_cast<uint32_t>(option("fa_v_lbo")) : FA_BN * 128;
-    p.v_sbo = option("fa_v_sbo") ? static_cast<uint32_t>(option("fa_v_sbo")) : 1024;
     p.poly_chunks = option("fa_poly");
-    // two query tiles per CTA (softmax of one tile overlaps the tensor-core work of the other) once that still
-    // fills the machine; GQA pairs two heads of a kv group at the same rows (identical causal extent and K/V tiles)
-    const bool pair_heads = (p.group % 2 == 0);
-    const long long ctas2 = pair_heads ? static_cast<long long>(p.n_qblk) * (Hq / 2) * B
-                                       : static_cast<long long>((p.n_qblk + 1) / 2) * Hq * B;
-    const int force = option("fa_nq");
-    const bool two = force ? (force == 2) : (ctas2 >= num_sms());
-    if (two) {
-        p.pair_heads = pair_heads ? 1 : 0;
-        dim3 grid(pair_heads ? p.n_qblk : (p.n_qblk + 1) / 2, pair_heads ? Hq / 2 : Hq, B);
-        return launch_flash_tc<DQK, DV, 2>(tmQ, tmK, tmV, p, grid, st);
-    }
-    p.pair_heads = 0;
     dim3 grid(p.n_qblk, Hq, B);
-    return launch_flash_tc<DQK, DV, 1>(tmQ, tmK, tmV, p, grid, st);
+    return launch_flash_tc<DQK, DV>(tmQ, tmK, tmV, p, grid, st);
 }
 
 }  // namespace vita

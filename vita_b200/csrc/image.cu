@@ -110,7 +110,7 @@ extern "C" int vita_image_tiles_lut(const uint8_t* img, const void* lut, void* o
     VITA_REQUIRE(gi > 0 && gj > 0 && T > 0 && tile0 >= 0, "image_tiles_lut: bad geometry");
     const long long n_pix = gi * gj * T * T;
     long long blocks = (n_pix + 255) / 256;
-    const long long cap = static_cast<long long>(num_sms() > 0 ? num_sms() : 148) * 16;
+    const long long cap = static_cast<long long>(num_sms() > 0 ? num_sms() : 132) * 16;
     if (blocks > cap) blocks = cap;
     image_tiles_lut_kernel<<<static_cast<unsigned>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         img, BF16C(lut), static_cast<__nv_bfloat16*>(out), static_cast<int>(gi), static_cast<int>(gj),

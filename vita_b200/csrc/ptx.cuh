@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA/TMEM).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor); the wgmma wrappers are in wgmma.cuh.
 // Everything here is device-only and header-only.
 #pragma once
 #include <cstdint>
@@ -43,8 +43,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     return ok != 0;
 }
 // Bounded wait: a protocol bug traps (kernel aborts with an error) instead of hanging the GPU.
+// The timeout message is a debug-build aid (-DVITA_MBAR_PRINT=1): a printf call anywhere in a kernel makes ptxas
+// serialise its wgmma.mma_async instructions.
+#ifndef VITA_MBAR_PRINT
+#define VITA_MBAR_PRINT 0
+#endif
 #ifndef VITA_MBAR_TIMEOUT_CYCLES
-#define VITA_MBAR_TIMEOUT_CYCLES (4000000000ll)  // ~2 s at 1.9 GHz
+#define VITA_MBAR_TIMEOUT_CYCLES (4000000000ll)  // ~2 s at the H100 boost clock
 #endif
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int tag = 0) {
     if (mbar_try_wait(bar, parity)) return;
@@ -52,13 +57,12 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int ta
     uint32_t spins = 0;
     while (!mbar_try_wait(bar, parity)) {
         if ((++spins & 0x3ff) == 0 && clock64() - t0 > VITA_MBAR_TIMEOUT_CYCLES) {
-            printf("[vita] mbarrier timeout: block %d thread %d tag %d parity %u\n", blockIdx.x, threadIdx.x, tag,
+            if (VITA_MBAR_PRINT) printf("[vita] mbarrier timeout: block %d thread %d tag %d parity %u\n", blockIdx.x, threadIdx.x, tag,
                    parity);
             __trap();
         }
     }
 }
-
 // ---------------------------------------------------------------- TMA
 // L2-only prefetch of one 2-D tile (no shared-memory destination, no barrier)
 __device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* m, int c0, int c1) {
@@ -91,115 +95,6 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
         "[%2];" ::"r"(smem_u32(smem_dst)),
         "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
         : "memory");
-}
-
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {  // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; bf16 inputs, fp32 accumulate.
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]: the A operand (M x 16 bf16, two K elements per 32-bit column) is read from
-// tensor memory, e.g. the softmax probabilities of an attention tile.
-__device__ __forceinline__ void tc_mma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                               uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets lane (base_lane + i), regs = columns.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM, same lane / column mapping as the loads above
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-          "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-          "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-          "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-          "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// UMMA shared-memory descriptor for a K-major bf16 tile stored as rows of 128 bytes with the 128B swizzle
-// (what TMA writes with CU_TENSOR_MAP_SWIZZLE_128B and a 64-element inner box).  8-row groups are 1024 B apart.
-// Field layout follows cute::UMMA::SmemDescriptor (version=1 for sm_100, layout_type 2 = SWIZZLE_128B).
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);  // start address, 16 B units
-    d |= static_cast<uint64_t>(1) << 16;                    // leading byte offset (unused for swizzled K-major)
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;            // stride byte offset: 8 rows * 128 B
-    d |= static_cast<uint64_t>(1) << 46;                    // descriptor version (Blackwell)
-    d |= static_cast<uint64_t>(2) << 61;                    // SWIZZLE_128B
-    return d;
-}
-// UMMA shared-memory descriptor for an MN-major bf16 operand with the 128B swizzle: rows of 128 bytes = 64 contiguous
-// elements along M/N, one row per K index (what TMA writes for a [K rows] x [64 MN columns] box), 8-row groups
-// 1024 B apart (stride byte offset); when the MN extent exceeds 64 the next 64-column block starts `lbo_bytes`
-// further (leading byte offset).  Canonical form ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
-    return d;
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): fp32 accum, bf16 A/B, both K-major, M x N tile.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(N >> 3) << 17) |
-           (static_cast<uint32_t>(M >> 4) << 24);
 }
 
 // ---------------------------------------------------------------- programmatic dependent launch
@@ -259,48 +154,22 @@ __device__ __forceinline__ float warp_max(float v) {
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
 }
-// packed 2 x fp32 arithmetic (FFMA2 / FADD2) and the 3-input maximum (FMNMX3) of sm_100: half the issue slots of the
-// scalar forms in the softmax inner loops
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rc, rd;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\t"
-        "fma.rn.f32x2 rd, ra, rb, rc;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-    return d;
-}
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rd;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\t"
-        "add.rn.f32x2 rd, ra, rb;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-    return d;
-}
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-    float d;
-    asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-    return d;
-}
 __device__ __forceinline__ float ex2_approx(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-// 2^x for a pair on the FMA / ALU pipes (no MUFU): round-to-nearest split x = n + f with the 1.5 * 2^23 trick, cubic
-// minimax of 2^f on [-0.5, 0.5] (relative error 7.5e-5, far below the bf16 rounding of the result), exponent insertion
-// by integer add.  x is clamped at -126 (anything smaller is 0 after the bf16 conversion anyway).
-__device__ __forceinline__ float2 ex2_poly2(float2 x) {
-    const float2 magic = make_float2(12582912.0f, 12582912.0f);
-    x.x = fmaxf(x.x, -126.0f);
-    x.y = fmaxf(x.y, -126.0f);
-    const float2 xr = fadd2(x, magic);
-    const float2 xi = fadd2(xr, make_float2(-12582912.0f, -12582912.0f));
-    const float2 f = fadd2(x, make_float2(-xi.x, -xi.y));
-    float2 p = ffma2(make_float2(0.05517162f, 0.05517162f), f, make_float2(0.24261113f, 0.24261113f));
-    p = ffma2(p, f, make_float2(0.69326097f, 0.69326097f));
-    p = ffma2(p, f, make_float2(0.99992806f, 0.99992806f));
-    p.x = __int_as_float(__float_as_int(p.x) + (__float_as_int(xr.x) << 23));
-    p.y = __int_as_float(__float_as_int(p.y) + (__float_as_int(xr.y) << 23));
-    return p;
+// 2^x on the FMA / ALU pipes (no MUFU): round-to-nearest split x = n + f with the 1.5 * 2^23 trick, cubic minimax of
+// 2^f on [-0.5, 0.5] (relative error 7.5e-5, far below the bf16 rounding of the result), exponent insertion by integer
+// add.  x is clamped at -126 (anything smaller is 0 after the bf16 conversion anyway).
+__device__ __forceinline__ float ex2_poly(float x) {
+    x = fmaxf(x, -126.0f);
+    const float xr = x + 12582912.0f;
+    const float f = x - (xr - 12582912.0f);
+    float p = fmaf(0.05517162f, f, 0.24261113f);
+    p = fmaf(p, f, 0.69326097f);
+    p = fmaf(p, f, 0.99992806f);
+    return __int_as_float(__float_as_int(p) + (__float_as_int(xr) << 23));
 }
 // rotate-half RoPE of one (x[j], x[j + D/2]) pair (transformers apply_rotary_pos_emb, modeling_mixtral.py:232-254).  One
 // definition for the stand-alone pass and the qkv GEMM epilogue, so both round identically.

@@ -1,4 +1,4 @@
-"""InternViT-300M vision tower on the B200 kernels.
+"""InternViT-300M vision tower on the CUDA kernels.
 
 Mirrors `InternViTVisionTower` (vita/model/multimodal_encoder/internvit/internvit_encoder.py:8-106) over
 `InternVisionModel` (modeling_intern_vit.py:321-394): same call signature and output ([N, 256, 4096] for 448 px tiles),

@@ -1,4 +1,4 @@
-"""Mixtral-8x7B sparse-MoE decoder on the B200 kernels: paged KV cache, prefill, CUDA-graphed greedy decode.
+"""Mixtral-8x7B sparse-MoE decoder on the CUDA kernels: paged KV cache, prefill, CUDA-graphed greedy decode.
 
 Replaces the third-party arithmetic the reference reaches through `self.model(...)` / `lm_head`
 (vita/model/language_model/vita_mixtral.py:158-173 -> transformers MixtralModel; vLLM twin
@@ -68,7 +68,7 @@ class MixtralDecoder:
         #   seq  (default) sequence-sharded residual stream: every rank owns S/N tokens for the dense part (qkv, causal
         #        attention over the all-gathered K/V, o-proj, router); K/V rows and routed activations are all-gathered
         #        and the expert outputs pushed to the token owners by P2P stores over NVLink symmetric memory
-        #   p2p  replicated dense part, fused P2P combine (round-1 design, kept as the A/B baseline)
+        #   p2p  replicated dense part, fused P2P combine (kept as the A/B baseline)
         #   nccl replicated dense part, partial sums + NCCL all-reduce (library baseline)
         self.ep_rank, self.ep_world = weights.get("ep", (0, 1))
         self.ep_mode = os.environ.get("VITA_B200_EP", "seq") if self.ep_world > 1 else None
@@ -98,7 +98,7 @@ class MixtralDecoder:
         self.d_act = torch.zeros(B, 2, I, dtype=BF16, device=dev)
         self.d_logits = torch.zeros(B, cfg.vocab_size, dtype=BF16, device=dev)
         self.attn_ws = ops.decode_attention_workspace(B, cfg.num_key_value_heads, self.decode_splits, dev)
-        # decode linears: tcgen05 swap-AB GEMVs (decode_tc.cu); their stream-K partial sums meet in one workspace
+        # decode linears: wgmma swap-AB GEMVs (decode_tc.cu); their stream-K partial sums meet in one workspace
         if H % 64 or I % 128:
             raise ValueError("the decode GEMVs need hidden_size % 64 == 0 and intermediate_size % 128 == 0")
         max_rb = max((cfg.vocab_size + 127) // 128, 2 * (I // 128), cfg.num_attention_heads
@@ -116,8 +116,8 @@ class MixtralDecoder:
         # (top-2 ids [T, 2] int32, renormalised weights [T, 2] fp32) pair per layer
         self.route_trace: Optional[list] = None
         # decode: the gate|up kernel can publish the expert pair as soon as its router is done so that the down projection
-        # streams its weight rows while gate|up is still running.  Bit-identical, but two same-box A/Bs measured it 0.7 %
-        # SLOWER (5.12 vs 5.08 and 5.27 vs 5.23 ms/token, profiles/r02_decode_ab.txt): off unless VITA_B200_EARLY_ROUTE=1
+        # streams its weight rows while gate|up is still running.  Bit-identical; not measured on H100:
+        # off unless VITA_B200_EARLY_ROUTE=1
         self.early_route = os.environ.get("VITA_B200_EARLY_ROUTE", "0") == "1"
         # prefill / batched decode: fused top-2 router + token permute over per-expert slot ranges (0 = align + gather)
         self.moe_fused = os.environ.get("VITA_B200_MOE_FUSED", "1") == "1"

@@ -1,4 +1,4 @@
-"""`VITAMixtralForCausalLM` on the B200 kernels -- the reference's Python surface for the omni forward path.
+"""`VITAMixtralForCausalLM` on the CUDA kernels -- the reference's Python surface for the omni forward path.
 
 Mirrors vita/model/language_model/vita_mixtral.py:232-415 + vita/model/vita_arch.py:111-407:
 `forward`, `generate`, `encode_images`, `encode_audios`, `prepare_inputs_labels_for_multimodal`, `get_vision_tower`,

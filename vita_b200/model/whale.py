@@ -1,4 +1,4 @@
-"""Whale audio encoder + CNNSubsampling adapter on the B200 kernels.
+"""Whale audio encoder + CNNSubsampling adapter on the CUDA kernels.
 
 Mirrors `audioEncoder.forward` (vita/model/multimodal_encoder/whale/init_model.py:114-139): fbank features
 [B, T, 80] + lengths [B] -> {"inputs_embeds": [B, T''', H_llm], "attention_mask": [B, T''']} with the shipped stack

@@ -365,7 +365,7 @@ def decode_router(h, norm_w, gate_w, xn, topk_ids, topk_w, eps):
               gate_w.shape[0], float(eps), _stream())
 
 
-# ------------------------------------------------------------------------------------------------ decode step (tcgen05)
+# ------------------------------------------------------------------------------------------------ decode step (wgmma)
 class TcWorkspace:
     """Cross-CTA reduction scratch of the tensor-core decode kernels (zero-initialised once, self-cleaning)."""
 

@@ -1,7 +1,7 @@
 """Multi-GPU plumbing: one process per GPU, torch.distributed for rendezvous and the few scalar reductions.
 
 Two ways the omni forward path shards (SURVEY.md section 8e):
-* by *request* (decode, short prompts): the whole model (93.7 GB bf16) fits one 180 GB B200, so each rank owns
+* by *request* (decode, short prompts): a 24-layer cut (70 GB bf16) fits one 80 GB H100, so each rank owns
   complete requests and their KV cache and the data path needs no collective; the only exchanges are bookkeeping
   (max-over-ranks timings, gathering generated token lists on rank 0);
 * by *expert and token* (one long sequence, BASELINE configs[3]): rank r holds experts [r E/N, (r+1) E/N) and owns the

@@ -1,4 +1,4 @@
-"""vLLM-facing model class on the B200 kernels (SURVEY.md section 8f rank 1, reference path B).
+"""vLLM-facing model class on the CUDA kernels (SURVEY.md section 8f rank 1, reference path B).
 
 Mirrors `MixtralForConditionalGeneration` of the reference's vLLM fork
 (web_demo/vllm_tools/vllm_file/mixtral.py:897-1330): `forward` over FLATTENED tokens with the engine's paged KV cache
