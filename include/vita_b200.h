@@ -243,6 +243,20 @@ int vita_decode_router(const void* h, const void* norm_w, const void* gate_w, vo
 int vita_decode_slots(const int32_t* cur_pos, const int32_t* block_table, int32_t* slots, int64_t B, int64_t page_size,
                       int64_t max_pages, void* stream);
 int vita_argmax_rows(const void* logits, uint64_t* best, int64_t B, int64_t V, void* stream);
+/* Sampled next token per row (temperature, top-k, top-p, Gumbel-max draw; the contract is stated in
+ * vita_b200/csrc/sample.cu and INTEGRATION.md section 2).  Replaces vLLM's Sampler at
+ * web_demo/vllm_tools/vllm_file/mixtral.py:1180-1186 and the sampling loop of HF generate() as called from
+ * video_audio_demo.py:257-270.  logits [B, ld] bf16 (first V columns); per-row device arrays temperature f32
+ * (0 = greedy: the packed word of vita_argmax_rows), top_k i32 (<= 0 or >= V: off), top_p f32 (>= 1: off),
+ * seed u64 (Philox key), counter i32 (index of the token being drawn within its request).  best [B]: packed
+ * (logit, ~index) like vita_argmax_rows.  scores (may be NULL): [B, score_rows, score_ld] bf16; row counter[b] of
+ * request b receives the warped row (x = l / T, -inf outside the kept set; the logits for greedy rows).
+ * V <= 82288 on an H100 (the row is staged in shared memory next to 64 KB of histograms).  Launched as a programmatic
+ * dependent: it waits for the preceding kernel before its first read of any input (the counter may be written by an
+ * earlier kernel of the same step) and lets its dependents start only when it has completed. */
+int vita_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
+                     const int32_t* top_k, const float* top_p, const uint64_t* seed, const int32_t* counter,
+                     uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows, void* stream);
 /* ---- greedy decode step on the tensor cores (wgmma swap-AB GEMV, stream-K) ---------------------------------
  * Every linear of the decode step as a weight-streaming GEMV on the tensor cores: the weight tile is the M operand of
  * wgmma and the activation vector as row 0 of a 16-wide N operand; (row-block, k-block) units are split evenly

@@ -1,0 +1,339 @@
+// Sampled next-token choice over bf16 logits (temperature, top-k, top-p, Gumbel-max draw), one CTA per row.
+//
+// Contract (vita_b200/sampling.py owns the policy; oracle/sampling_oracle.py restates it in fp64):
+//   T == 0 (or negative) -> greedy: the packed (logit, ~index) word of argmax_rows, first index on ties
+//   x_r = l_r / T in fp32 from the bf16 logit
+//   top-k (0 < k < V): keep every token whose logit is >= the k-th largest (boundary ties kept)
+//   top-p (p < 1): over the softmax of the top-k survivors keep r iff the mass of the survivors whose logit is strictly
+//                  greater than l_r is < p (tied values are kept or dropped together); the largest logit always stays
+//   draw: argmax_r over the kept set of x_r + g_r (lowest index on ties), g_r = -log(-log(u_r)),
+//         u_r = ((w >> 8) + 0.5) * 2^-24, w = word (r & 3) of Philox4x32-10(counter (r >> 2, n, 0, 0),
+//         key (seed lo, seed hi)), n = counter[b]
+// Logits are bf16 and the temperature is monotone, so both thresholds are found by radix selection over the 16-bit
+// ordered keys of the logits (two 256-bin passes each): top-k over counts, top-p over fixed-point masses
+// exp(x_r - x_max) * 2^40 summed as u64 (integer sums: the result does not depend on the order of the additions).
+//
+// Reference call sites: vLLM's Sampler (web_demo/vllm_tools/vllm_file/mixtral.py:1180-1186) and the sampling loop of
+// HF generate() (video_audio_demo.py:257-270: TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper ->
+// multinomial).
+#include "common.h"
+#include "ptx.cuh"
+
+namespace vita {
+
+constexpr int kSampleThreads = 1024;
+constexpr int kSampleWarps = kSampleThreads / 32;
+constexpr size_t kSampleHistBytes = static_cast<size_t>(kSampleWarps) * 256 * 8;   // per-warp 256-bin histograms
+
+// bf16 bits <-> 16-bit key whose unsigned order is the numeric order (the order pack_argmax induces on floats)
+__device__ __forceinline__ uint32_t bf16_key(uint32_t u) { return (u & 0x8000u) ? (~u & 0xFFFFu) : (u | 0x8000u); }
+__device__ __forceinline__ float key_value(uint32_t k) {
+    const uint32_t u = (k & 0x8000u) ? (k & 0x7FFFu) : (~k & 0xFFFFu);
+    return __uint_as_float(u << 16);
+}
+__device__ __forceinline__ unsigned long long pack_score(float v, int idx) {
+    uint32_t u = __float_as_uint(v);
+    u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+    return (static_cast<unsigned long long>(u) << 32) | static_cast<unsigned long long>(0xFFFFFFFFu - static_cast<uint32_t>(idx));
+}
+
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        if (r) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+        const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+    }
+    return c;
+}
+
+// g = -log(-log(u)), u = ((w >> 8) + 0.5) * 2^-24.  -log(u) is taken as -log1p(-(1 - u)) in the upper half, where
+// 1 - u = ((2^24 - 1 - (w >> 8)) + 0.5) * 2^-24 is exact in fp32 (u itself is not: it would round to 1 at the top).
+__device__ __forceinline__ float gumbel(uint32_t w) {
+    const uint32_t a = w >> 8;
+    const float nl = a < (1u << 23) ? -logf((static_cast<float>(a) + 0.5f) * 0x1p-24f)
+                                    : -log1pf(-(static_cast<float>(0xFFFFFFu - a) + 0.5f) * 0x1p-24f);
+    return -logf(nl);
+}
+// Bounds of g over all 2^24 values of u: [-2.8527, 17.3287].  A token whose x is more than their spread (plus fp32
+// slack) below x_max can never beat the largest logit's perturbed score, so it needs no noise.
+constexpr float kGumbelPrune = 24.0f;
+
+__device__ __forceinline__ unsigned long long block_max_u64(unsigned long long v, unsigned long long* red) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long other = __shfl_xor_sync(0xffffffffu, v, o);
+        v = other > v ? other : v;
+    }
+    __syncthreads();                                    // red may still be read from a previous reduction
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        v = red[threadIdx.x];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const unsigned long long other = __shfl_xor_sync(0xffffffffu, v, o);
+            v = other > v ? other : v;
+        }
+        if (threadIdx.x == 0) red[0] = v;
+    }
+    __syncthreads();
+    return red[0];
+}
+
+// Histogram over the keys >= floor_key: high bytes (hi_bin < 0) or the low bytes of the keys whose high byte is
+// hi_bin.  Weight 1 (counts) or the fixed-point mass exp(x - x_max) * 2^40.  Result in tot[256].
+__device__ void sample_hist(const uint16_t* keys, int V, unsigned long long* whist, unsigned long long* tot,
+                            int hi_bin, uint32_t floor_key, bool mass, float T, float x_max) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    unsigned long long* h = whist + warp * 256;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) h[lane + 32 * j] = 0ull;
+    __syncwarp();
+    for (int i = threadIdx.x; i < V; i += kSampleThreads) {
+        const uint32_t k = keys[i];
+        if (k < floor_key) continue;
+        if (hi_bin >= 0 && static_cast<int>(k >> 8) != hi_bin) continue;
+        unsigned long long wt = 1ull;
+        if (mass) {
+            const float x = __fdiv_rn(key_value(k), T);
+            wt = __float2ull_rn(expf(x - x_max) * 0x1p40f);
+            if (wt == 0ull) continue;
+        }
+        atomicAdd(h + (hi_bin < 0 ? (k >> 8) : (k & 255u)), wt);
+    }
+    __syncthreads();
+    if (threadIdx.x < 256) {
+        unsigned long long s = 0ull;
+        for (int w = 0; w < kSampleWarps; ++w) s += whist[w * 256 + threadIdx.x];
+        tot[threadIdx.x] = s;
+    }
+    __syncthreads();
+}
+
+// Warp 0: the lowest bin b with base + (weight of the bins above b) < target.  The qualifying bins form a run from
+// the top, so that is where the run ends.  Writes {bin or -1, weight above it} to res; res_total = sum of all bins.
+__device__ void sample_search(const unsigned long long* tot, unsigned long long base, double target, int* res_bin,
+                              unsigned long long* res_above, unsigned long long* res_total) {
+    if (threadIdx.x >= 32) return;
+    const int lane = threadIdx.x;
+    unsigned long long s = 0ull;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s += tot[255 - 8 * lane - j];       // lane 0 owns the 8 highest bins
+    unsigned long long incl = s;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += v;
+    }
+    unsigned long long above = base + incl - s;
+    int last = -1;
+    unsigned long long last_above = 0ull;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const int b = 255 - 8 * lane - j;
+        if (static_cast<double>(above) < target) { last = b; last_above = above; }
+        above += tot[b];
+    }
+    const unsigned mask = __ballot_sync(0xffffffffu, last >= 0);
+    const unsigned long long total = __shfl_sync(0xffffffffu, incl, 31);
+    if (mask == 0u) {
+        if (lane == 0) { *res_bin = -1; *res_above = 0ull; *res_total = total; }
+        return;
+    }
+    const int src = 31 - __clz(static_cast<int>(mask));
+    const int bin = __shfl_sync(0xffffffffu, last, src);
+    const unsigned long long ab = __shfl_sync(0xffffffffu, last_above, src);
+    if (lane == 0) { *res_bin = bin; *res_above = ab; *res_total = total; }
+}
+
+__global__ void __launch_bounds__(kSampleThreads, 1)
+sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, const float* __restrict__ temperature,
+                   const int* __restrict__ top_k, const float* __restrict__ top_p,
+                   const unsigned long long* __restrict__ seed, const int* __restrict__ counter,
+                   unsigned long long* __restrict__ best, __nv_bfloat16* __restrict__ scores, long long score_ld,
+                   int score_rows, int vec) {
+    extern __shared__ __align__(16) uint8_t smem_s[];
+    unsigned long long* whist = reinterpret_cast<unsigned long long*>(smem_s);
+    uint16_t* keys = reinterpret_cast<uint16_t*>(smem_s + kSampleHistBytes);
+    __shared__ unsigned long long tot[256];
+    __shared__ unsigned long long red[32];
+    __shared__ int s_bin;
+    __shared__ unsigned long long s_above, s_total;
+
+    const int b = blockIdx.x;
+    const int tid = threadIdx.x;
+    // Nothing is read before the wait: the logits come from the preceding kernel, and the counter (the decoder's
+    // gen_count) is written on the device earlier in the same step by a kernel that triggers its dependents before
+    // that write -- only griddepcontrol.wait makes it visible, whatever the chain options.
+    pdl_wait();
+    const float T = temperature[b];
+    const int k = top_k[b];
+    const float p = top_p[b];
+    const unsigned long long key = seed[b];
+    const int n = counter[b];
+
+    // stage the row as ordered keys; greedy arg-max on the way (largest key, first index)
+    const __nv_bfloat16* row = logits + static_cast<long long>(b) * ld;
+    uint32_t bk = 0u;
+    int bi = 0x7fffffff;
+    if (vec) {
+        for (int j = tid; j < (V >> 3); j += kSampleThreads) {
+            const uint4 q = __ldg(reinterpret_cast<const uint4*>(row) + j);
+            const uint32_t w4[4] = {q.x, q.y, q.z, q.w};
+            uint32_t kk[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const uint32_t lo = bf16_key(w4[e] & 0xFFFFu), hi = bf16_key(w4[e] >> 16);
+                kk[e] = lo | (hi << 16);
+                const int i = 8 * j + 2 * e;
+                if (lo > bk || (lo == bk && i < bi)) { bk = lo; bi = i; }
+                if (hi > bk || (hi == bk && i + 1 < bi)) { bk = hi; bi = i + 1; }
+            }
+            reinterpret_cast<uint4*>(keys)[j] = make_uint4(kk[0], kk[1], kk[2], kk[3]);
+        }
+    } else {
+        const uint16_t* r16 = reinterpret_cast<const uint16_t*>(row);
+        for (int i = tid; i < V; i += kSampleThreads) {
+            const uint32_t kk = bf16_key(r16[i]);
+            keys[i] = static_cast<uint16_t>(kk);
+            if (kk > bk || (kk == bk && i < bi)) { bk = kk; bi = i; }
+        }
+    }
+    const unsigned long long arg = block_max_u64(bi == 0x7fffffff ? 0ull : pack_score(key_value(bk), bi), red);
+    const bool greedy = !(T > 0.0f);
+    __nv_bfloat16* srow = nullptr;
+    if (scores != nullptr && n >= 0 && n < score_rows)
+        srow = scores + (static_cast<long long>(b) * score_rows + n) * score_ld;
+
+    if (greedy) {                                        // bit-identical to argmax_rows; the score log gets the logits
+        if (tid == 0) best[b] = arg;
+        if (srow != nullptr)
+            for (int i = tid; i < V; i += kSampleThreads) srow[i] = __float2bfloat16(key_value(keys[i]));
+        return;
+    }
+    const uint32_t ord = static_cast<uint32_t>(arg >> 32);     // undo pack_score's float ordering, then re-key
+    const uint32_t max_key = bf16_key(((ord & 0x80000000u) ? (ord & 0x7FFFFFFFu) : ~ord) >> 16);
+    const float x_max = __fdiv_rn(key_value(max_key), T);
+
+    // top-k threshold: the k-th largest key
+    uint32_t thr = 0u;
+    if (k > 0 && k < V) {
+        sample_hist(keys, V, whist, tot, -1, 0u, false, T, x_max);
+        sample_search(tot, 0ull, static_cast<double>(k), &s_bin, &s_above, &s_total);
+        __syncthreads();
+        const int hb = s_bin;
+        const unsigned long long ab = s_above;
+        sample_hist(keys, V, whist, tot, hb, 0u, false, T, x_max);
+        sample_search(tot, ab, static_cast<double>(k), &s_bin, &s_above, &s_total);
+        __syncthreads();
+        thr = (static_cast<uint32_t>(hb) << 8) | static_cast<uint32_t>(s_bin);
+    }
+    // top-p threshold over the top-k survivors: the lowest key whose strictly-greater survivor mass is < p * Z
+    if (p < 1.0f) {
+        sample_hist(keys, V, whist, tot, -1, thr, true, T, x_max);
+        if (tid < 32) {                                  // Z = survivor mass = sum of all bins
+            unsigned long long s = 0ull;
+            for (int j = tid; j < 256; j += 32) s += tot[j];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            if (tid == 0) s_total = s;
+        }
+        __syncthreads();
+        const double target = static_cast<double>(p) * static_cast<double>(s_total);
+        __syncthreads();                                 // s_total is rewritten by the search
+        sample_search(tot, 0ull, target, &s_bin, &s_above, &s_total);
+        __syncthreads();
+        const int hb = s_bin;
+        const unsigned long long ab = s_above;
+        uint32_t tp = max_key;                           // nothing qualifies (p == 0): the largest logit stays
+        if (hb >= 0) {
+            sample_hist(keys, V, whist, tot, hb, thr, true, T, x_max);
+            sample_search(tot, ab, target, &s_bin, &s_above, &s_total);
+            __syncthreads();
+            tp = (static_cast<uint32_t>(hb) << 8) | static_cast<uint32_t>(s_bin < 0 ? 0 : s_bin);
+        }
+        thr = tp > thr ? tp : thr;
+    }
+
+    // Gumbel-max over the kept keys (>= thr)
+    const float x_floor = x_max - kGumbelPrune;
+    const uint32_t k0 = static_cast<uint32_t>(key), k1 = static_cast<uint32_t>(key >> 32);
+    unsigned long long loc = 0ull;
+    const int n_groups = (V + 3) >> 2;
+    for (int j = tid; j < n_groups; j += kSampleThreads) {
+        float x[4];
+        bool kept[4], need = false;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int i = 4 * j + e;
+            const uint32_t kk = i < V ? keys[i] : 0u;
+            kept[e] = i < V && kk >= thr;
+            x[e] = __fdiv_rn(key_value(kk), T);
+            need |= kept[e] && x[e] >= x_floor;
+            if (srow != nullptr && i < V) srow[i] = kept[e] ? __float2bfloat16(x[e]) : __float2bfloat16(-INFINITY);
+        }
+        if (!need) continue;
+        const uint4 w = philox4x32_10(make_uint4(static_cast<uint32_t>(j), static_cast<uint32_t>(n), 0u, 0u), k0, k1);
+        const uint32_t ww[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            if (!kept[e] || x[e] < x_floor) continue;
+            const unsigned long long s = pack_score(x[e] + gumbel(ww[e]), 4 * j + e);
+            loc = s > loc ? s : loc;
+        }
+    }
+    const unsigned long long win = block_max_u64(loc, red);
+    // the winner's packed word keeps the arg-max layout: (bf16 logit as float, ~index)
+    if (tid == 0) {
+        const int idx = static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(win & 0xFFFFFFFFull));
+        best[b] = pack_score(key_value(keys[idx]), idx);
+    }
+}
+
+}  // namespace vita
+
+using namespace vita;
+
+extern "C" int vita_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
+                                const int32_t* top_k, const float* top_p, const uint64_t* seed, const int32_t* counter,
+                                uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows, void* stream) {
+    VITA_REQUIRE(V > 0 && ld >= V, "need 0 < V <= ld");
+    VITA_REQUIRE(temperature && top_k && top_p && seed && counter && best, "parameter arrays are required");
+    VITA_REQUIRE(scores == nullptr || (score_ld >= V && score_rows > 0), "score log: need score_ld >= V, rows > 0");
+    if (B == 0) return VITA_OK;
+    // dynamic shared memory available = the device's opt-in per-block limit minus the kernel's static shared memory
+    // (on an H100: 232448 - 2336 bytes, which leaves V <= 82288 next to the 64 KB of histograms)
+    static size_t dyn_limit = 0;
+    if (dyn_limit == 0) {
+        int dev = 0, optin = 0;
+        cudaFuncAttributes fa{};
+        int rc = check_cuda(cudaGetDevice(&dev), "sample_rows");
+        if (!rc) rc = check_cuda(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev), "sample_rows");
+        if (!rc) rc = check_cuda(cudaFuncGetAttributes(&fa, sample_rows_kernel), "sample_rows");
+        if (rc) return rc;
+        dyn_limit = static_cast<size_t>(optin) > fa.sharedSizeBytes ? static_cast<size_t>(optin) - fa.sharedSizeBytes : 0;
+    }
+    const size_t smem = kSampleHistBytes + ((static_cast<size_t>(V) * 2 + 15) / 16) * 16;
+    VITA_REQUIRE(smem <= dyn_limit, "the row does not fit shared memory (V <= " +
+                                        std::to_string(dyn_limit > kSampleHistBytes ? (dyn_limit - kSampleHistBytes) / 16 * 8 : 0) +
+                                        " on this device)");
+    static size_t configured = 0;
+    if (smem > configured) {
+        const int rc = check_cuda(cudaFuncSetAttribute(sample_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                       static_cast<int>(smem)), "sample_rows");
+        if (rc) return rc;
+        configured = smem;
+    }
+    const int vec = (V % 8 == 0 && ld % 8 == 0 && aligned16(logits)) ? 1 : 0;
+    // launched as a programmatic dependent of the LM head: the kernel waits (griddepcontrol.wait) before reading the
+    // logits and never triggers its own dependents early, so the next step starts after its last write of `best`
+    cudaError_t e = launch_chain(sample_rows_kernel, dim3(static_cast<unsigned>(B)), dim3(kSampleThreads), smem,
+                                 static_cast<cudaStream_t>(stream), BF16C(logits), (long long)ld, (int)V, temperature,
+                                 top_k, top_p, reinterpret_cast<const unsigned long long*>(seed), counter,
+                                 reinterpret_cast<unsigned long long*>(best), static_cast<__nv_bfloat16*>(scores),
+                                 (long long)score_ld, (int)score_rows, vec);
+    if (e != cudaSuccess) return check_cuda(e, "sample_rows");
+    return check_launch("sample_rows");
+}

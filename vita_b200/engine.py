@@ -32,6 +32,8 @@ from typing import Callable, Dict, List, Optional, Sequence
 
 import torch
 
+from .sampling import SamplingParams
+
 
 @dataclass
 class Request:
@@ -42,6 +44,7 @@ class Request:
     arrival_step: int = 0               # engine step at which the request becomes visible
     session: Optional[int] = None       # duplex: queries of one conversation; a real query interrupts the running answer
     negative_token_id: Optional[int] = None   # duplex: state token `<2>`; a query answering with it is dropped at once
+    sampling: Optional[SamplingParams] = None  # None = greedy (vita_b200/sampling.py: from_hf / from_vllm build one)
     # filled in by the batcher
     outcome: str = ""                   # "finished" | "negative" | "interrupted"
     steps: int = 0
@@ -152,7 +155,7 @@ class DecoderEngine:
         self.lone_fast_path = lone_fast_path
         c = self.llm.cache
         self._slot_tensors = [c.block_table, c.slot_map, c.cache_len, c.cur_pos, self.llm.best, self.llm.token_log,
-                              self.llm.gen_count]
+                              self.llm.gen_count, *self.llm.sampling.tensors]
 
     def reset_slot(self, slot: int) -> None:
         c = self.llm.cache
@@ -167,16 +170,21 @@ class DecoderEngine:
         if need > self.llm.cache.max_seq_len or request.max_new_tokens > self.llm.max_new_tokens:
             raise ValueError(f"request {request.rid}: {need} KV positions / {request.max_new_tokens} new tokens exceed "
                              f"the engine's capacity ({self.llm.cache.max_seq_len} / {self.llm.max_new_tokens})")
-        self.llm.prefill(emb[0, : lens[0]].contiguous(), slot=slot)
+        self.llm.sampling.set(slot, request.sampling)
+        self.llm.prefill(emb[0, : lens[0]].contiguous(), slot=slot, sampled=request.sampling is not None)
 
     def step(self, n_active: int) -> None:
+        # the sampled step when any active request samples (its greedy rows keep the greedy tokens), else the greedy one
+        sampled = self.llm.sampling.any_sampled(n_active)
         if n_active == 1 and self.lone_fast_path:      # a lone request takes the weight-streaming GEMV chain (2 experts read, not a GEMM tile)
-            self.llm.decode_step(1, use_graph=self.use_graph)
+            self.llm.decode_step(1, use_graph=self.use_graph, sampled=sampled)
         else:
-            self.llm.decode_step_batched(n_active, use_graph=self.use_graph)
+            self.llm.decode_step_batched(n_active, use_graph=self.use_graph, sampled=sampled)
 
     def swap(self, i: int, j: int) -> None:
         swap_rows(self._slot_tensors, i, j)
+        if i != j:
+            self.llm.sampling.swap(i, j)
 
     def read_tokens(self, slot: int) -> List[int]:
         return self.llm.generated_tokens(slot)

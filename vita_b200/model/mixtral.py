@@ -1,4 +1,4 @@
-"""Mixtral-8x7B sparse-MoE decoder on the CUDA kernels: paged KV cache, prefill, CUDA-graphed greedy decode.
+"""Mixtral-8x7B sparse-MoE decoder on the CUDA kernels: paged KV cache, prefill, CUDA-graphed greedy or sampled decode.
 
 Replaces the third-party arithmetic the reference reaches through `self.model(...)` / `lm_head`
 (vita/model/language_model/vita_mixtral.py:158-173 -> transformers MixtralModel; vLLM twin
@@ -13,6 +13,7 @@ import torch
 
 from .. import ops
 from ..config import LLMConfig
+from ..sampling import SlotSampling
 
 BF16 = torch.bfloat16
 
@@ -88,6 +89,7 @@ class MixtralDecoder:
         self.best = torch.zeros(B, dtype=torch.int64, device=dev)         # packed (logit, ~index) arg-max
         self.token_log = torch.zeros(B, max_new_tokens + 8, dtype=torch.int32, device=dev)
         self.gen_count = torch.zeros(B, dtype=torch.int32, device=dev)
+        self.sampling = SlotSampling(B, dev)                              # per-slot sampler parameters
         self.d_h = torch.zeros(B, H, dtype=BF16, device=dev)
         self.d_q = torch.zeros(B, cfg.num_attention_heads * cfg.head_dim, dtype=BF16, device=dev)
         self.d_attn = torch.zeros_like(self.d_q)
@@ -106,9 +108,9 @@ class MixtralDecoder:
         self.tc_ws = ops.TcWorkspace(B, max_rb, dev)
         # completion counters of the bs = 1 decode chain: [serial, one counter per chain kernel (5 per layer + LM head)]
         self.chain_mem = torch.zeros(2 + 5 * cfg.num_hidden_layers, dtype=torch.int64, device=dev)
-        self._graphs = {}             # single-sequence decode step: captured CUDA graph per (B, want_logits)
+        self._graphs = {}             # single-sequence decode step: captured CUDA graph per (B, want_logits[, sampled])
         self.scores_buf = None        # [max_new_tokens + 1, V] logits log of slot 0 (generate(output_scores=True))
-        self._bgraphs = {}            # batched decode step: captured CUDA graph per batch size
+        self._bgraphs = {}            # batched decode step: captured CUDA graph per (batch size, sampled)
         self.d_slots = torch.zeros(B, dtype=torch.int32, device=dev)
         self._prefill_ws = {}
         # router decisions of every layer (the reference returns them as `router_logits` when asked,
@@ -236,16 +238,21 @@ class MixtralDecoder:
 
     @torch.no_grad()
     def prefill(self, inputs_embeds: torch.Tensor, slot: int = 0, all_logits: bool = False,
-                want_last_logits: bool = False):
+                want_last_logits: bool = False, sampled: bool = False, scores: Optional[torch.Tensor] = None):
         """One sequence: inputs_embeds [S, H] bf16 (consumed as the residual stream, modified in place).
 
         Appends S tokens to the KV cache of batch slot `slot` (which must be empty), leaves the arg-max of the last
-        position in self.best[slot] (the first generated token) and returns logits [S, V] if `all_logits`."""
+        position in self.best[slot] (the first generated token) and returns logits [S, V] if `all_logits`.
+        `sampled`: the first token is drawn instead (self.sampling's parameters of the slot, counter 0 =
+        gen_count[slot] of the empty slot) from the last-row logits; `scores` [rows, V] receives the warped row at
+        row 0."""
         c, w = self.cfg, self.w
         S, H = inputs_embeds.shape
         assert inputs_embeds.dtype == BF16 and inputs_embeds.is_cuda and inputs_embeds.is_contiguous()
         if S > self.cache.max_seq_len:
             raise ValueError(f"prompt of {S} tokens exceeds the KV capacity of {self.cache.max_seq_len} per sequence")
+        if sampled and self.ep_world > 1:
+            raise ValueError("sampled decoding is single-GPU: the expert-parallel prefill serves greedy requests")
         if self.ep_mode == "seq":
             return self._prefill_ep_seq(inputs_embeds, slot, all_logits, want_last_logits)
         ws = self._ws(S)
@@ -326,9 +333,11 @@ class MixtralDecoder:
         self.cache.cache_len[slot:slot + 1] += S
         # first generated token: final norm + lm_head + arg-max on the last row only
         self.best[slot:slot + 1].zero_()
-        last_logits = self.d_logits[slot:slot + 1] if (want_last_logits or all_logits) else None
+        last_logits = self.d_logits[slot:slot + 1] if (want_last_logits or all_logits or sampled) else None
         ops.tc_lm_head_argmax(h[S - 1:], H, w["norm"], w["lm_head"], last_logits, self.best[slot:slot + 1], 1,
                               self.tc_ws, c.rms_norm_eps)
+        if sampled:
+            self._sample(slot, 1, scores)
         if all_logits:
             return ops.linear(xn, w["lm_head"])      # [S, V]; xn = final RMSNorm(h) written by the last combine
         return last_logits
@@ -411,10 +420,12 @@ class MixtralDecoder:
         return last_logits
 
     # ------------------------------------------------------------------------------------------ decode
-    def _decode_step_kernels(self, B: int, want_logits: bool):
+    def _decode_step_kernels(self, B: int, want_logits: bool, sampled: bool = False):
         """One greedy token for slots [0, B): embed + per layer (qkv+RoPE+KV append -> paged attention -> o-proj ->
         router+gate/up -> down) + LM head with arg-max, 2 + 5 L launches chained by programmatic dependent launch.
-        For B = 1 the kernels are additionally linked by completion counters (include/vita_b200.h, vita_chain_begin)."""
+        For B = 1 the kernels are additionally linked by completion counters (include/vita_b200.h, vita_chain_begin).
+        `sampled`: the LM head writes the logits and the sampler draws the token from them (one launch more, after the
+        counter chain; with a score log it writes the warped row in place of the logits copy)."""
         c, w, cache = self.cfg, self.w, self.cache
         nq, nkv, D = c.num_attention_heads, c.num_key_value_heads, c.head_dim
         h = self.d_h[:B]
@@ -440,12 +451,21 @@ class MixtralDecoder:
                 if tracing:
                     self.route_trace.append((self.d_ids[:B].clone(), self.d_w[:B].clone()))
                 ops.decode_tc_moe_down(self.d_act[:B], lw["w2"], self.d_ids[:B], self.d_w[:B], h, ws, route, li + 1)
-            lg = self.d_logits[:B] if want_logits else None
+            lg = self.d_logits[:B] if (want_logits or sampled) else None
             ops.tc_lm_head_argmax(h, c.hidden_size, w["norm"], w["lm_head"], lg, self.best[:B], B, ws, c.rms_norm_eps)
         finally:
             if chained:
                 ops.chain_end()
-        self._log_scores(B, want_logits)
+        if sampled:
+            self._sample(0, B, self.scores_buf if (want_logits and B == 1) else None)
+        else:
+            self._log_scores(B, want_logits)
+
+    def _sample(self, s0: int, n: int, scores: Optional[torch.Tensor]):
+        """Draw the next token of slots [s0, s0 + n) from d_logits into best (counter = gen_count of the slot)."""
+        sp, rows = self.sampling, slice(s0, s0 + n)
+        ops.sample_rows(self.d_logits[rows], sp.temperature[rows], sp.top_k[rows], sp.top_p[rows], sp.seed[rows],
+                        self.gen_count[rows], self.best[rows], scores)
 
     def enable_score_log(self):
         """Allocate the per-step logits log (HF `output_scores=True`): row i holds the logits token i was chosen from.
@@ -469,22 +489,28 @@ class MixtralDecoder:
     def launches_per_decode_step_with_scores(self) -> int:
         return self.launches_per_decode_step + 1
 
-    @torch.no_grad()
-    def decode_step(self, B: int = 1, use_graph: bool = True, want_logits: bool = False):
-        assert self.ep_world == 1, "expert-parallel mode covers the prefill (BASELINE configs[3]); decode is replicated"
-        self._decode_step(B, use_graph, want_logits)
+    @property
+    def launches_per_decode_step_sampled(self) -> int:
+        """A sampled bs = 1 step, with or without the score log: the sampler replaces the logits copy."""
+        return self.launches_per_decode_step + 1
 
-    def _decode_step(self, B: int = 1, use_graph: bool = True, want_logits: bool = False):
+    @torch.no_grad()
+    def decode_step(self, B: int = 1, use_graph: bool = True, want_logits: bool = False, sampled: bool = False):
+        assert self.ep_world == 1, "expert-parallel mode covers the prefill (BASELINE configs[3]); decode is replicated"
+        self._decode_step(B, use_graph, want_logits, sampled)
+
+    def _decode_step(self, B: int = 1, use_graph: bool = True, want_logits: bool = False, sampled: bool = False):
         """Generate one token for batch slots [0, B): consumes self.best, appends to token_log, leaves the next
-        arg-max in self.best.  With use_graph the whole step (2 + 5 * layers kernels) replays as one CUDA graph."""
+        arg-max (or, `sampled`, the drawn token) in self.best.  With use_graph the whole step (2 + 5 * layers kernels,
+        one more when sampled) replays as one CUDA graph."""
         if not use_graph:
-            self._decode_step_kernels(B, want_logits)
+            self._decode_step_kernels(B, want_logits, sampled)
             return
-        key = (B, want_logits)
+        key = (B, want_logits, True) if sampled else (B, want_logits)    # greedy keys keep their (B, want_logits) form
         if key not in self._graphs:
             # capture (the kernels were warmed up by an eager step so every cudaFuncSetAttribute already ran)
             self._snapshot = self._save_state()
-            self._decode_step_kernels(B, want_logits)
+            self._decode_step_kernels(B, want_logits, sampled)
             torch.cuda.synchronize()
             self._restore_state(self._snapshot)
             g = torch.cuda.CUDAGraph()
@@ -492,7 +518,7 @@ class MixtralDecoder:
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
                 with torch.cuda.graph(g, stream=side):
-                    self._decode_step_kernels(B, want_logits)
+                    self._decode_step_kernels(B, want_logits, sampled)
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
             self._restore_state(self._snapshot)   # capture does not execute, but keep the invariant explicit
@@ -500,7 +526,7 @@ class MixtralDecoder:
         self._graphs[key].replay()
 
     # ------------------------------------------------------------------------------------------ batched decode
-    def _batched_step_kernels(self, B: int, want_logits: bool):
+    def _batched_step_kernels(self, B: int, want_logits: bool, sampled: bool = False):
         """One token for each of B sequences through the GEMM path (weights of every touched expert are streamed once
         for the whole batch; BASELINE configs[4]).  Same kernels as the prefill, with M = B rows at B different
         positions, + the paged decode attention."""
@@ -542,21 +568,25 @@ class MixtralDecoder:
             ops.moe_down(act, lw["w2"], yp, ws["offs"], rw, 2 * B)
             ops.moe_combine(h, yp, perm, nxt, xn, c.rms_norm_eps)
         logits = ops.linear(xn, w["lm_head"], out=self.d_logits[:B])
-        ops.argmax_rows(logits, self.best[:B])
+        if sampled:          # greedy rows (temperature 0) get argmax_rows' word: a mixed batch keeps their tokens
+            self._sample(0, B, None)
+        else:
+            ops.argmax_rows(logits, self.best[:B])
 
     @property
     def launches_per_batched_step(self) -> int:
         return (6 + 8 * self.cfg.num_hidden_layers) if self.moe_fused else (5 + 10 * self.cfg.num_hidden_layers)
 
     @torch.no_grad()
-    def decode_step_batched(self, B: int, use_graph: bool = True):
+    def decode_step_batched(self, B: int, use_graph: bool = True, sampled: bool = False):
         assert self.ep_world == 1 and 1 <= B <= self.max_batch
         if not use_graph:
-            self._batched_step_kernels(B, False)
+            self._batched_step_kernels(B, False, sampled)
             return
-        if B not in self._bgraphs:             # one captured graph per batch size (continuous batching changes B)
+        key = (B, sampled)
+        if key not in self._bgraphs:           # one captured graph per batch size (continuous batching changes B)
             snap = self._save_state()
-            self._batched_step_kernels(B, False)          # warm-up (cudaFuncSetAttribute etc.)
+            self._batched_step_kernels(B, False, sampled)  # warm-up (cudaFuncSetAttribute etc.)
             torch.cuda.synchronize()
             self._restore_state(snap)
             g = torch.cuda.CUDAGraph()
@@ -564,12 +594,12 @@ class MixtralDecoder:
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
                 with torch.cuda.graph(g, stream=side):
-                    self._batched_step_kernels(B, False)
+                    self._batched_step_kernels(B, False, sampled)
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
             self._restore_state(snap)
-            self._bgraphs[B] = g
-        self._bgraphs[B].replay()
+            self._bgraphs[key] = g
+        self._bgraphs[key].replay()
 
     def _save_state(self):
         c = self.cache

@@ -15,6 +15,7 @@ import torch
 from .. import ops
 from ..config import VitaConfig, IMAGE_TOKEN_INDEX, AUDIO_TOKEN_INDEX
 from .internvit import InternViTVisionTower, VisionProjector
+from ..sampling import from_hf
 from .mixtral import MixtralDecoder
 from .whale import AudioEncoder
 
@@ -329,22 +330,28 @@ class VITAMixtralForCausalLM:
 
     @torch.no_grad()
     def generate_batch(self, requests, max_new_tokens: int = 16, use_graph: bool = True, step_callback=None):
-        """Concurrent greedy decode of several independent requests (BASELINE configs[4]: duplex / bs=16 streaming).
+        """Concurrent decode of several independent requests (BASELINE configs[4]: duplex / bs=16 streaming).
 
-        `requests`: list of dicts {"input_ids": [1, L], "images": ..., "audios": ...}.  Each request is prefilled
-        into its own paged-KV slot, then all of them advance one token per step through the batched decode step.
-        Returns the list of generated token lists.  `step_callback(step_index)` is called after every step launch
-        (latency harnesses record CUDA events there)."""
+        `requests`: list of dicts {"input_ids": [1, L], "images": ..., "audios": ...}, optionally with
+        "sampling": {"temperature", "top_k", "top_p", "seed"} (as for generate(do_sample=True)); the others are greedy.
+        Each request is prefilled into its own paged-KV slot, then all of them advance one token per step through the
+        batched decode step.  Returns the list of generated token lists.  `step_callback(step_index)` is called after
+        every step launch (latency harnesses record CUDA events there)."""
         B = len(requests)
         if not 1 <= B <= self.llm.max_batch:
             raise ValueError(f"{B} requests do not fit max_batch = {self.llm.max_batch}")
+        params = [None if r.get("sampling") is None else from_hf(True, **r["sampling"]) for r in requests]
+        if any(params) and self.llm.ep_world > 1:
+            raise ValueError("sampled decoding is single-GPU (the expert-parallel mode serves greedy requests)")
         self.llm.reset()
         for b, r in enumerate(requests):
             emb, lens = self._embeds_for(r["input_ids"], r.get("images"), r.get("audios"))
             self.llm.check_capacity(lens[0], max_new_tokens)
-            self.llm.prefill(emb[0, : lens[0]].contiguous(), slot=b)
+            self.llm.sampling.set(b, params[b])
+            self.llm.prefill(emb[0, : lens[0]].contiguous(), slot=b, sampled=params[b] is not None)
+        sampled = any(p is not None for p in params)
         for step in range(max_new_tokens):
-            self.llm.decode_step_batched(B, use_graph=use_graph)
+            self.llm.decode_step_batched(B, use_graph=use_graph, sampled=sampled)
             if step_callback is not None:
                 step_callback(step)
         return [self.llm.generated_tokens(b)[:max_new_tokens] for b in range(B)]
@@ -395,24 +402,36 @@ class VITAMixtralForCausalLM:
     def generate(self, input_ids, images=None, audios=None, do_sample=False, temperature=None, top_p=None,
                  num_beams=1, output_scores=False, return_dict_in_generate=True, max_new_tokens=16, use_cache=True,
                  stopping_criteria=None, eos_token_id: Optional[int] = None, use_graph: bool = True, sync_every: int = 16,
-                 **kw):
-        """Greedy decode with the call signature of video_audio_demo.py:257-270.  `sequences` (on `input_ids.device`)
-        echoes the prompt ids, placeholders included, followed by the new tokens (video_audio_demo.py:272-276).
+                 top_k=None, seed: Optional[int] = None, **kw):
+        """Greedy or sampled decode with the call signature of video_audio_demo.py:257-270.  `sequences` (on
+        `input_ids.device`) echoes the prompt ids, placeholders included, followed by the new tokens
+        (video_audio_demo.py:272-276).
+
+        `do_sample=True` draws every token, the first one included, with `temperature`, `top_k`, `top_p` (None = HF
+        4.41's defaults 1.0, 50, 1.0; the policy is vita_b200/sampling.py).  `seed` (an extension) is the 64-bit stream
+        key; without it one key is drawn from torch's default CPU generator, so `torch.manual_seed` makes a call
+        reproducible.  With `output_scores` the scores are the warped rows, as HF returns them when sampling.
 
         The decode step replays as one CUDA graph whether or not `output_scores` is set: with scores the step appends
         its logits row to a device-resident log, and `scores` are views of that log (valid until the next call).
         Tokens are read back every `sync_every` steps; stopping criteria see each new token exactly once."""
-        if do_sample or num_beams != 1:
-            raise ValueError("the hot path is greedy decode (do_sample=False, num_beams=1)")
+        if num_beams != 1:
+            raise ValueError("beam search is not supported (num_beams=1)")
+        params = from_hf(do_sample, temperature, top_k, top_p, seed, **kw)
+        sampled = params is not None
+        if sampled and self.llm.ep_world > 1:
+            raise ValueError("sampled decoding is single-GPU (the expert-parallel mode serves greedy requests)")
         if input_ids.shape[0] != 1:
             raise ValueError("generate() is single-sequence like the demo; use generate_batch() for more")
         emb, lens = self._embeds_for(input_ids, images, audios)
         llm = self.llm
         llm.check_capacity(lens[0], max_new_tokens)
         llm.reset()
+        llm.sampling.set(0, params)
         score_log = llm.enable_score_log() if output_scores else None
-        first = llm.prefill(emb[0, : lens[0]].contiguous(), slot=0, want_last_logits=output_scores)
-        if output_scores:
+        first = llm.prefill(emb[0, : lens[0]].contiguous(), slot=0, want_last_logits=output_scores, sampled=sampled,
+                            scores=score_log)
+        if output_scores and not sampled:
             score_log[0].copy_(first[0])
         prompt = input_ids[0].tolist()
         L = len(prompt)
@@ -423,7 +442,7 @@ class VITAMixtralForCausalLM:
         while step < max_new_tokens and not done:
             n = min(sync_every, max_new_tokens - step)
             for _ in range(n):
-                llm.decode_step(1, use_graph=use_graph, want_logits=output_scores)
+                llm.decode_step(1, use_graph=use_graph, want_logits=output_scores, sampled=sampled)
             step += n
             toks = llm.generated_tokens(0)[:max_new_tokens]     # one host sync per `sync_every` tokens
             n_new = len(toks)

@@ -164,6 +164,33 @@ def argmax_rows(logits, best):
     _lib.call("vita_argmax_rows", _p(logits), _p(best), logits.shape[0], logits.shape[1], _stream())
 
 
+def sample_rows(logits, temperature, top_k, top_p, seed, counter, best, scores: Optional[torch.Tensor] = None):
+    """Sampled next token per row into the packed arg-max words `best` (contract: vita_b200/sampling.py).
+    logits [B, V] bf16 (rows may be strided); temperature / top_p f32 [B], top_k / counter i32 [B], seed i64 [B]
+    (the 64-bit Philox key, bit pattern); scores [B, rows, V] or [rows, V] (B = 1) bf16: row counter[b] receives
+    the warped logits."""
+    _chk(logits, BF16, "logits", contiguous=False); _chk(best, torch.int64, "best")
+    _chk(temperature, torch.float32, "temperature"); _chk(top_p, torch.float32, "top_p")
+    _chk(top_k, torch.int32, "top_k"); _chk(counter, torch.int32, "counter"); _chk(seed, torch.int64, "seed")
+    B, V = logits.shape
+    if logits.stride(1) != 1:
+        raise _lib.VitaB200Error("sample_rows: logits rows must be contiguous")
+    for t, n in ((temperature, "temperature"), (top_k, "top_k"), (top_p, "top_p"), (seed, "seed"),
+                 (counter, "counter"), (best, "best")):
+        if t.numel() < B:
+            raise _lib.VitaB200Error(f"sample_rows: {n} has fewer than {B} rows")
+    rows = 0
+    if scores is not None:
+        _chk(scores, BF16, "scores")
+        if scores.dim() == 2:
+            scores = scores.unsqueeze(0)
+        if scores.shape[0] < B or scores.shape[2] != V:
+            raise _lib.VitaB200Error("sample_rows: scores must be [B, rows, V]")
+        rows = scores.shape[1]
+    _lib.call("vita_sample_rows", _p(logits), logits.stride(0), B, V, _p(temperature), _p(top_k), _p(top_p),
+              _p(seed), _p(counter), _p(best), _p(scores), V, rows, _stream())
+
+
 # ------------------------------------------------------------------------------------------------ MoE (prefill)
 def moe_router(h, norm_w, gate_w, xn, topk_ids, topk_w, eps):
     _chk(h, BF16, "h"); _chk(norm_w, BF16, "norm_w"); _chk(gate_w, BF16, "gate_w"); _chk(xn, BF16, "xn")

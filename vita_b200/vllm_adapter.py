@@ -3,7 +3,7 @@
 Mirrors `MixtralForConditionalGeneration` of the reference's vLLM fork
 (web_demo/vllm_tools/vllm_file/mixtral.py:897-1330): `forward` over FLATTENED tokens with the engine's paged KV cache
 (:1130-1172), `merge_multimodal_embeddings` (:1084-1128, placeholder ids -> feature rows, in place), `compute_logits`
-(:1174-1178), greedy `sample` (:1180-1186) and `load_weights` with the checkpoint -> kernel name map (:1189-1330).
+(:1174-1178), `sample` (:1180-1186; greedy or sampled per sequence group) and `load_weights` with the checkpoint -> kernel name map (:1189-1330).
 
 What the engine hands the model per step is captured by `TokenBatch` (the fields of vLLM's flash-attention metadata:
 slot mapping, block tables, sequence / query lengths); the engine's block tables and KV tensors are used as they are --
@@ -27,6 +27,7 @@ import torch
 
 from . import ops, weights as W
 from .config import VitaConfig
+from .sampling import from_vllm, row_tensors
 from .model.internvit import InternViTVisionTower, VisionProjector
 from .model.mixtral import MixtralDecoder
 from .model.whale import AudioEncoder
@@ -232,9 +233,42 @@ class MixtralForConditionalGeneration:
 
     @torch.no_grad()
     def sample(self, logits: torch.Tensor, sampling_metadata=None) -> torch.Tensor:
-        """Greedy next tokens (the reference demos sample with temperature 0.001, web_ability_demo.py:353)."""
-        best = torch.zeros(logits.shape[0], dtype=torch.int64, device=logits.device)
-        ops.argmax_rows(logits.contiguous(), best)
+        """Next token per logits row.  With vLLM 0.5.5's SamplingMetadata, each sequence group that samples
+        (`do_sample`, default True) draws the rows `sample_indices` points at (its position in `seq_groups` when the
+        field is absent and there is one row per group) from `sampling_params`: temperature < 1e-5 is greedy,
+        otherwise the row is drawn (vita_b200/sampling.py) with the request's seed as key and counter = the output
+        length of its sequence (`seq_data[id].get_output_len()`); unseeded rows take one key each from torch's default
+        generator.  Every other row -- a group that does not sample (a chunked-prefill chunk), prompt-logprob rows --
+        and every row of a call without metadata (or without `seq_groups`) gets the greedy arg-max, as before (the
+        reference demos sample with temperature 0.001 / 0.01, web_interactive_demo.py:132, web_ability_demo.py:351)."""
+        B = logits.shape[0]
+        best = torch.zeros(B, dtype=torch.int64, device=logits.device)
+        groups = getattr(sampling_metadata, "seq_groups", None)
+        if groups is None:
+            ops.argmax_rows(logits.contiguous(), best)
+            return (0xFFFFFFFF - (best & 0xFFFFFFFF)).to(torch.int64)
+        params, counter = [None] * B, [0] * B
+        for i, sg in enumerate(groups):
+            if not getattr(sg, "do_sample", True):
+                continue
+            rows = getattr(sg, "sample_indices", None)
+            if rows is None:
+                if len(groups) != B:
+                    raise ValueError(f"{len(groups)} sequence groups without sample_indices for {B} logits rows")
+                rows = [i]
+            rows = [int(r) for r in rows]
+            if not rows:
+                continue
+            ids = list(sg.seq_ids)
+            if len(ids) != 1 or len(rows) != 1:
+                raise NotImplementedError("sequence groups with several sequences (n > 1, beam search)")
+            if not 0 <= rows[0] < B:
+                raise ValueError(f"sample index {rows[0]} outside the {B} logits rows")
+            params[rows[0]] = from_vllm(sg.sampling_params)
+            counter[rows[0]] = int(sg.seq_data[ids[0]].get_output_len())
+        T, K, P, S = row_tensors(params, logits.device)
+        cnt = torch.tensor(counter, dtype=torch.int32).to(logits.device, non_blocking=True)
+        ops.sample_rows(logits.contiguous(), T, K, P, S, cnt, best)
         return (0xFFFFFFFF - (best & 0xFFFFFFFF)).to(torch.int64)
 
 
