@@ -102,6 +102,21 @@ int vita_attention_fwd(const void* q, const void* k, const void* v, void* o, con
                        const int64_t* k_strides, const int64_t* v_strides, const int64_t* o_strides, int64_t B,
                        int64_t n_q_heads, int64_t n_kv_heads, int64_t Sq, int64_t Skv, int64_t d_qk, int64_t d_v,
                        const int32_t* kv_lens, int causal, int64_t q_pos0, float scale, void* stream);
+/* causal attention of prompt continuations over a paged KV cache: sequence i owns the packed query rows
+ * [query_start_loc[i], query_start_loc[i + 1]) (C_i rows of q, token stride q_token_stride, heads head_dim apart) and
+ * ctx_lens[i] = P_i + C_i keys in the pages block_table[i * bt_stride ...], its own keys already appended; row r
+ * attends keys <= P_i + r.  k_cache / v_cache: [n_slots, n_kv_heads, head_dim], slot = page * page_size + offset.
+ * tiles: n_tiles pairs (sequence, 128-row query block), one CTA per pair and q head, in launch order (longest rows
+ * first is fastest).  Pages past ceil(ctx_lens[i] / page_size) are never read; keys at positions >= ctx_lens[i] never
+ * reach the output.  The same rows through vita_attention_fwd over the gathered keys give bit-identical output.
+ * head_dim 128, page_size 16 / 32 / 64 / 128.  Replaces vLLM's paged attention in MixtralAttention.forward
+ * (web_demo/vllm_tools/vllm_file/mixtral.py:484-501) when a prefill continues cached blocks (chunked prefill,
+ * prefix caching). */
+int vita_attention_prefill_paged(const void* q, int64_t q_token_stride, const void* k_cache, const void* v_cache,
+                                 int64_t n_slots, const int32_t* block_table, int64_t bt_stride,
+                                 const int32_t* query_start_loc, const int32_t* ctx_lens, const int32_t* tiles,
+                                 int64_t n_tiles, void* out, int64_t o_token_stride, int64_t T, int64_t n_q_heads,
+                                 int64_t n_kv_heads, int64_t head_dim, int64_t page_size, float scale, void* stream);
 /* single-query paged-KV attention for decode (vLLM paged Attention, mixtral.py:484-501).  workspace must be
  * zero-initialised once and be at least vita_decode_attention_workspace_bytes() large for the largest (B, splits) it
  * is used with; every launch hands it back all-zero, so B and splits may change from call to call.  The context

@@ -7,6 +7,8 @@ greedy decode; reports p50 / p99 inter-token latency and tokens/s.  (8 x H100 = 
                                                         # continuous batcher, with duplex events (negative-audio abort,
                                                         # barge-in interrupt); under torchrun the 16 queries are sharded
                                                         # over the ranks (request parallel) and the latencies gathered
+    python scripts/bench_cfg5.py --arrivals 12 --prefill-chunk 512   # the same mix plus one video-length (4096-token)
+                                                        # arrival, run without and with chunked admission (one GPU)
 """
 import argparse
 import json
@@ -39,8 +41,9 @@ def run_arrivals(args):
     B, NT = args.batch, args.new_tokens
     mine = parallel.shard_requests(B, rank, world)
     packed = W.random_packed(cfg, dev, seed=0, parts=("llm", "vision", "projector", "audio"))
-    model = VITAMixtralForCausalLM(cfg, packed, dev, max_batch=max(len(mine), 1), max_seq_len=512 + NT + 16,
-                                   max_new_tokens=NT + 16)
+    long_len = 4096 if args.prefill_chunk else 0
+    model = VITAMixtralForCausalLM(cfg, packed, dev, max_batch=max(len(mine), 1) + (1 if long_len else 0),
+                                   max_seq_len=max(512, long_len) + NT + 16, max_new_tokens=NT + 16)
     rng = random.Random(7)
     g = torch.Generator().manual_seed(0)
     reqs, t = [], 0
@@ -53,6 +56,13 @@ def run_arrivals(args):
                    "audios": {"audios": torch.randn(1, 998, 80, generator=g), "lengths": torch.tensor([998])}}
         # sessions of 2 queries each: the second query of a session barges in on the first one's answer
         reqs.append(Request(b, payload, NT, None, arrival_step=t, session=b // 2, negative_token_id=cfg.llm.vocab_size - 1))
+    if long_len:
+        # an 8-frame video conversation turn (S ~ 4096; text rows stand in for the spliced frame features, the prefill
+        # cost is the same), arriving in the middle of the mix
+        assert world == 1, "--prefill-chunk measures one GPU"
+        ids = torch.randint(0, cfg.llm.vocab_size - 8, (1, long_len), generator=g)
+        reqs.append(Request(B, {"input_ids": ids}, NT, None, arrival_step=reqs[B // 2].arrival_step))
+        mine = list(mine) + [B]
     my_reqs = [r for r in reqs if r.rid in mine]
     eng = DecoderEngine(model, use_graph=True, overrun=8, lone_fast_path=True)
     # warm-up: every batch size this rank will see gets its graph captured outside the measurement
@@ -62,25 +72,45 @@ def run_arrivals(args):
     torch.cuda.synchronize()
     if world > 1:
         dist.barrier()
-    marks = []
-    start = torch.cuda.Event(enable_timing=True)
-    start.record()
 
-    def on_step(step, n_active):
-        e = torch.cuda.Event(enable_timing=True)
-        e.record()
-        marks.append((step, n_active, e))
+    def measure(chunk):
+        marks = []
+        start = torch.cuda.Event(enable_timing=True)
+        start.record()
 
-    out = ContinuousBatcher(eng, max(len(mine), 1), sync_every=8).run(my_reqs, on_step=on_step)
-    torch.cuda.synchronize()
-    ts = [(st, n, start.elapsed_time(e)) for st, n, e in marks]
-    itl = []                                            # one sample per (step, active request)
-    for (s0, n0, t0), (s1, n1, t1) in zip(ts, ts[1:]):
-        itl += [t1 - t0] * n1
-    total_tokens = sum(len(v) for v in out.values())
-    wall_ms = ts[-1][2] if ts else 0.0
-    rec = {"itl": itl, "tokens": total_tokens, "wall_ms": wall_ms,
-           "outcomes": [r.outcome for r in my_reqs], "steps": len(ts)}
+        def on_step(step, n_active):
+            e = torch.cuda.Event(enable_timing=True)
+            e.record()
+            marks.append((step, n_active, e))
+
+        for r in my_reqs:
+            r.steps, r.tokens, r.outcome = 0, [], ""
+        out = ContinuousBatcher(eng, max(len(mine), 1), sync_every=8, prefill_chunk=chunk).run(my_reqs, on_step=on_step)
+        torch.cuda.synchronize()
+        ts = [(st, n, start.elapsed_time(e)) for st, n, e in marks]
+        itl = []                                            # one sample per (step, active request)
+        for (s0, n0, t0), (s1, n1, t1) in zip(ts, ts[1:]):
+            itl += [t1 - t0] * n1
+        total_tokens = sum(len(v) for v in out.values())
+        wall_ms = ts[-1][2] if ts else 0.0
+        return {"itl": itl, "tokens": total_tokens, "wall_ms": wall_ms,
+                "outcomes": [r.outcome for r in my_reqs], "steps": len(ts)}
+
+    if long_len:
+        q = lambda v, p: sorted(v)[min(len(v) - 1, int(len(v) * p))]
+        res = {}
+        for chunk in (None, args.prefill_chunk):
+            r = measure(chunk)
+            res["whole" if chunk is None else f"chunk_{chunk}"] = {
+                "p50_itl_ms": q(r["itl"], 0.5), "p99_itl_ms": q(r["itl"], 0.99), "max_itl_ms": max(r["itl"]),
+                "tokens_per_s": r["tokens"] / (r["wall_ms"] / 1e3), "steps": r["steps"]}
+        print(json.dumps({
+            "workload": f"configs[4] arrivals (mean gap {args.arrivals} steps) plus one {long_len}-token arrival, "
+                        f"{NT} new tokens each, {args.layers} layers, 1 GPU: arrivals prefilled whole vs. chunked "
+                        f"admission with a budget of {args.prefill_chunk} tokens per step",
+            "gpu": torch.cuda.get_device_name(), "power_limit": _power_limit(), **res}))
+        return
+    rec = measure(None)
     allrec = [None] * world
     if world > 1:
         dist.all_gather_object(allrec, rec)
@@ -106,12 +136,24 @@ def run_arrivals(args):
         dist.destroy_process_group()
 
 
+def _power_limit() -> str:
+    import subprocess
+    try:
+        return subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                               str(torch.cuda.current_device())], capture_output=True, text=True,
+                              timeout=30).stdout.strip() or "unknown"
+    except Exception:
+        return "unknown"
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=16)
     ap.add_argument("--new-tokens", type=int, default=256)
     ap.add_argument("--layers", type=int, default=32)
     ap.add_argument("--arrivals", type=float, default=0.0, help="mean gap between arrivals in decode steps (0 = all at step 0)")
+    ap.add_argument("--prefill-chunk", type=int, default=None,
+                    help="with --arrivals: add a 4096-token arrival and compare whole against chunked admission")
     args = ap.parse_args()
     if args.arrivals > 0:
         return run_arrivals(args)

@@ -30,6 +30,8 @@ SIGNATURES = {
     "vita_rope_kv_write": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, P]),
     "vita_gemm_qkv_rope": (c_int, [P, I64, P, P, I64, I64, I64, I64, I64, P, P, P, P, P, P]),
     "vita_attention_fwd": (c_int, [P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P, c_int, I64, c_float, P]),
+    "vita_attention_prefill_paged": (c_int, [P, I64, P, P, I64, P, I64, P, P, P, I64, P, I64, I64, I64, I64, I64, I64,
+                                             c_float, P]),
     "vita_decode_attention_workspace_bytes": (I64, [I64, I64, I64]),
     "vita_decode_attention": (c_int, [P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, c_float, I64, P]),
     "vita_decode_slots": (c_int, [P, P, P, I64, I64, I64, P]),

@@ -14,6 +14,15 @@
 //   Mixtral causal GQA 128/128  transformers sdpa / eager attention (modeling_mixtral.py:269-292)
 //   InternViT non-causal 64/64  flash_attn_varlen_qkvpacked_func (internvit/flash_attention.py:61)
 //   Whale rel-pos 128/64        attention.py:391-415, both score terms as one contraction over [k | p], key padding
+//
+// The PAGED instantiation (Mixtral 128/128, causal) continues sequences whose keys sit in a paged KV cache: prompt
+// chunks and prompts whose prefix is cached (vLLM's paged attention in MixtralAttention.forward, mixtral.py:484-501,
+// when a prefill continues cached blocks).  Only the producer and the per-CTA set-up differ: a CTA takes its
+// (sequence, query block) from a host-built tile list, and a K / V tile of 128 keys arrives as one TMA box per page and
+// per 64-column half.  Pages start at multiples of 16 rows (2048 B), so the 128B-swizzled shared-memory image is the
+// one the single 128-row box of the contiguous path writes, and the consumers run unchanged.  V rows at positions
+// >= ctx (stale page tails, pages never loaded) are zeroed before the P V product; masked scores alone would leave
+// 0 * NaN.
 #include "common.h"
 #include "ptx.cuh"
 #include "wgmma.cuh"
@@ -31,6 +40,14 @@ struct FaParams {
     float scale_log2;             // softmax scale * log2(e)
     int n_qblk;                   // number of 128-row query blocks
     int poly_chunks;              // of the 4 column chunks of a tile, how many take exp2 on the FMA pipe (MUFU relief)
+    // PAGED: CTA blockIdx.x serves tiles[2 blockIdx.x ..] = (sequence i, query block); sequence i owns packed query
+    // rows [qsl[i], qsl[i + 1]) and ctx[i] keys (its cached prefix and the rows themselves) in the pages block_table[i]
+    const int* tiles;             // int32 pairs: 4-byte alignment only
+    const int* qsl;
+    const int* ctx;
+    const int* block_table;
+    int bt_stride;
+    int page_shift;               // log2(page_size)
 };
 
 constexpr int FA_BM = 128;   // query rows per tile (64 per consumer warpgroup)
@@ -46,7 +63,7 @@ struct FaCfg {
     static constexpr int SMEM = Q_BYTES + STAGES * (K_BYTES + V_BYTES) + 1024 /*align*/ + 256 /*barriers*/;
 };
 
-template <int DQK, int DV, int POLY>
+template <int DQK, int DV, int POLY, bool PAGED>
 __global__ void __launch_bounds__(FaCfg<DQK, DV>::THREADS, 1)
 flash_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FaParams p) {
@@ -67,27 +84,46 @@ flash_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     uint64_t* v_empty = v_full + ST;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int b = blockIdx.z;
-
-    // long causal rows first
-    const int bx = p.causal ? static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x) : static_cast<int>(blockIdx.x);
     const int head = blockIdx.y;
-    const int q0 = bx * FA_BM;
     const int kvh = head / p.group;
-    int kv_len = p.kv_lens ? p.kv_lens[b] : p.Skv;
-    if (kv_len > p.Skv) kv_len = p.Skv;
-    if (kv_len < 0) kv_len = 0;
+    int b, q0, Sq, q_pos0, kv_len, q_row0;   // q_row0: TMA row coordinate of query row q0
+    __nv_bfloat16* obase;                     // output row 0 of this (batch entry | sequence)
+    const int* bt = nullptr;
+    if constexpr (PAGED) {
+        const int seq = p.tiles[2 * blockIdx.x];   // the host orders the list long causal rows first
+        const int r0 = p.qsl[seq];
+        b = 0;
+        q0 = p.tiles[2 * blockIdx.x + 1] * FA_BM;
+        Sq = p.qsl[seq + 1] - r0;
+        kv_len = p.ctx[seq];
+        q_pos0 = kv_len - Sq;
+        q_row0 = r0 + q0;
+        obase = p.o + static_cast<long long>(r0) * p.o_ts;
+        bt = p.block_table + static_cast<long long>(seq) * p.bt_stride;
+    } else {
+        b = blockIdx.z;
+        // long causal rows first
+        const int bx = p.causal ? static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x) : static_cast<int>(blockIdx.x);
+        q0 = bx * FA_BM;
+        Sq = p.Sq;
+        q_pos0 = p.q_pos0;
+        kv_len = p.kv_lens ? p.kv_lens[b] : p.Skv;
+        if (kv_len > p.Skv) kv_len = p.Skv;
+        if (kv_len < 0) kv_len = 0;
+        q_row0 = q0;
+        obase = nullptr;   // p.o + b * p.o_bs, formed where it is used (keeps this instantiation's code as it was)
+    }
     int n_tiles = (kv_len + FA_BN - 1) / FA_BN;
     if (p.causal) {
-        const int lim = (p.q_pos0 + q0 + FA_BM + FA_BN - 1) / FA_BN;   // keys <= last row of the tile
+        const int lim = (q_pos0 + q0 + FA_BM + FA_BN - 1) / FA_BN;   // keys <= last row of the tile
         if (n_tiles > lim) n_tiles = lim;
     }
 
     if (n_tiles == 0) {   // no keys at all: zeros (uniform over the CTA)
         if (threadIdx.x >= 128 && threadIdx.x < 128 + FA_BM) {
             const int row = q0 + static_cast<int>(threadIdx.x) - 128;
-            if (row < p.Sq) {
-                uint4* orow = reinterpret_cast<uint4*>(p.o + b * p.o_bs + static_cast<long long>(row) * p.o_ts + head * p.o_hs);
+            if (row < Sq) {
+                uint4* orow = reinterpret_cast<uint4*>((PAGED ? obase : p.o + b * p.o_bs) + static_cast<long long>(row) * p.o_ts + head * p.o_hs);
                 for (int i = 0; i < DV / 8; ++i) orow[i] = make_uint4(0, 0, 0, 0);
             }
         }
@@ -116,21 +152,55 @@ flash_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         if (threadIdx.x == 0) {
             mbar_arrive_expect_tx(q_full, Cfg::Q_BYTES);
 #pragma unroll
-            for (int c = 0; c < DQK / 64; ++c) tma_load_4d(sQ + c * HALF, &tmQ, q_full, c * 64, q0, head, b);
+            for (int c = 0; c < DQK / 64; ++c) tma_load_4d(sQ + c * HALF, &tmQ, q_full, c * 64, q_row0, head, b);
             int stage = 0;
             uint32_t phase = 0;
-            for (int j = 0; j < n_tiles; ++j) {
-                mbar_wait(&k_empty[stage], phase ^ 1, 10);
-                mbar_arrive_expect_tx(&k_full[stage], Cfg::K_BYTES);
+            if constexpr (PAGED) {
+                // tmK / tmV: [slots][n_kv][D] with a box of {64, 1, page_size}; pages past ctx are never read
+                constexpr int MAXPG = FA_BN / 16;
+                const int ps = 1 << p.page_shift;
+                const int ppt = FA_BN >> p.page_shift;   // pages per key tile
+                for (int j = 0; j < n_tiles; ++j) {
+                    const int pg0 = j * ppt;
+                    const int npg = min(ppt, ((kv_len + ps - 1) >> p.page_shift) - pg0);
+                    int slot0[MAXPG];
 #pragma unroll
-                for (int c = 0; c < DQK / 64; ++c)
-                    tma_load_4d(sK + stage * Cfg::K_BYTES + c * HALF, &tmK, &k_full[stage], c * 64, j * FA_BN, kvh, b);
-                mbar_wait(&v_empty[stage], phase ^ 1, 11);
-                mbar_arrive_expect_tx(&v_full[stage], Cfg::V_BYTES);
+                    for (int g = 0; g < MAXPG; ++g) slot0[g] = g < npg ? bt[pg0 + g] << p.page_shift : 0;
+                    const uint32_t rows = static_cast<uint32_t>(npg) << p.page_shift;
+                    mbar_wait(&k_empty[stage], phase ^ 1, 10);
+                    mbar_arrive_expect_tx(&k_full[stage], rows * DQK * 2);
 #pragma unroll
-                for (int c = 0; c < DV / 64; ++c)
-                    tma_load_4d(sV + stage * Cfg::V_BYTES + c * HALF, &tmV, &v_full[stage], c * 64, j * FA_BN, kvh, b);
-                if (++stage == ST) { stage = 0; phase ^= 1; }
+                    for (int g = 0; g < MAXPG; ++g)
+                        if (g < npg)
+#pragma unroll
+                            for (int c = 0; c < DQK / 64; ++c)
+                                tma_load_3d(sK + stage * Cfg::K_BYTES + c * HALF + g * ps * 128, &tmK, &k_full[stage],
+                                            c * 64, kvh, slot0[g]);
+                    mbar_wait(&v_empty[stage], phase ^ 1, 11);
+                    mbar_arrive_expect_tx(&v_full[stage], rows * DV * 2);
+#pragma unroll
+                    for (int g = 0; g < MAXPG; ++g)
+                        if (g < npg)
+#pragma unroll
+                            for (int c = 0; c < DV / 64; ++c)
+                                tma_load_3d(sV + stage * Cfg::V_BYTES + c * HALF + g * ps * 128, &tmV, &v_full[stage],
+                                            c * 64, kvh, slot0[g]);
+                    if (++stage == ST) { stage = 0; phase ^= 1; }
+                }
+            } else {
+                for (int j = 0; j < n_tiles; ++j) {
+                    mbar_wait(&k_empty[stage], phase ^ 1, 10);
+                    mbar_arrive_expect_tx(&k_full[stage], Cfg::K_BYTES);
+#pragma unroll
+                    for (int c = 0; c < DQK / 64; ++c)
+                        tma_load_4d(sK + stage * Cfg::K_BYTES + c * HALF, &tmK, &k_full[stage], c * 64, j * FA_BN, kvh, b);
+                    mbar_wait(&v_empty[stage], phase ^ 1, 11);
+                    mbar_arrive_expect_tx(&v_full[stage], Cfg::V_BYTES);
+#pragma unroll
+                    for (int c = 0; c < DV / 64; ++c)
+                        tma_load_4d(sV + stage * Cfg::V_BYTES + c * HALF, &tmV, &v_full[stage], c * 64, j * FA_BN, kvh, b);
+                    if (++stage == ST) { stage = 0; phase ^= 1; }
+                }
             }
         }
         return;
@@ -171,11 +241,11 @@ flash_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
         // ---- softmax on the fragment: s[4 jb + 2 h + e] is row[h], key col0 + 8 jb + 2 qc + e
         const int col0 = j * FA_BN;
-        const bool boundary = (col0 + FA_BN > kv_len) || (p.causal && col0 + FA_BN - 1 > p.q_pos0 + wg_q0);   // warp-uniform
+        const bool boundary = (col0 + FA_BN > kv_len) || (p.causal && col0 + FA_BN - 1 > q_pos0 + wg_q0);   // warp-uniform
         if (boundary) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int lim = p.causal ? min(kv_len, p.q_pos0 + row[h] + 1) : kv_len;   // columns >= lim are masked
+                const int lim = p.causal ? min(kv_len, q_pos0 + row[h] + 1) : kv_len;   // columns >= lim are masked
 #pragma unroll
                 for (int jb = 0; jb < FA_BN / 8; ++jb)
 #pragma unroll
@@ -222,6 +292,19 @@ flash_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         // ---- O += P V_j: 16 keys per instruction, P from registers, V rows of 128 B as an MN-major operand (64-column
         // blocks FA_BN * 128 B apart, 8-key groups 1024 B apart)
         mbar_wait(&v_full[stage], phase, 22);
+        if constexpr (PAGED) {
+            if (col0 + FA_BN > kv_len) {   // CTA-uniform: zero V rows [kv_len - col0, FA_BN) (both consumer warpgroups)
+                const int r_lo = kv_len - col0;
+                const int n = (FA_BN - r_lo) * (DV / 8);   // 16-byte chunks; a row is 128 B in each 64-column half
+                uint8_t* vt = sV + stage * Cfg::V_BYTES;
+                for (int i = static_cast<int>(threadIdx.x) - 128; i < n; i += 256) {
+                    const int r = r_lo + i / (DV / 8), c = i % (DV / 8);
+                    *reinterpret_cast<uint4*>(vt + (c >> 3) * HALF + r * 128 + (c & 7) * 16) = make_uint4(0, 0, 0, 0);
+                }
+                fence_proxy_async_smem();
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+            }
+        }
         wgmma_acc_fence(o);
         wgmma_fence();
 #pragma unroll
@@ -239,14 +322,20 @@ flash_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     }
 
     // ---- epilogue: O / l -> bf16 -> global
+    if constexpr (PAGED) {   // re-read rather than keep live through the loop (register pressure of the POLY variant)
+        const int seq = p.tiles[2 * blockIdx.x];
+        const int r0 = p.qsl[seq];
+        Sq = p.qsl[seq + 1] - r0;
+        obase = p.o + static_cast<long long>(r0) * p.o_ts;
+    }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         float lt = l[h];
         lt += __shfl_xor_sync(0xffffffffu, lt, 1);
         lt += __shfl_xor_sync(0xffffffffu, lt, 2);
         const float inv = lt > 0.0f ? 1.0f / lt : 0.0f;
-        if (row[h] < p.Sq) {
-            __nv_bfloat16* orow = p.o + b * p.o_bs + static_cast<long long>(row[h]) * p.o_ts + head * p.o_hs;
+        if (row[h] < Sq) {
+            __nv_bfloat16* orow = (PAGED ? obase : p.o + b * p.o_bs) + static_cast<long long>(row[h]) * p.o_ts + head * p.o_hs;
 #pragma unroll
             for (int jb = 0; jb < DV / 8; ++jb)
                 *reinterpret_cast<uint32_t*>(orow + jb * 8 + 2 * qc) = pack_bf16(o[4 * jb + 2 * h] * inv, o[4 * jb + 2 * h + 1] * inv);
@@ -254,12 +343,12 @@ flash_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     }
 }
 
-template <int DQK, int DV, int POLY>
+template <int DQK, int DV, int POLY, bool PAGED>
 static int launch_flash_tc_p(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const FaParams& p,
                              dim3 grid, cudaStream_t st) {
     using Cfg = FaCfg<DQK, DV>;
     static bool configured = false;
-    auto kern = flash_tc_kernel<DQK, DV, POLY>;
+    auto kern = flash_tc_kernel<DQK, DV, POLY, PAGED>;
     if (!configured) {
         int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM),
                             "cudaFuncSetAttribute(flash_tc smem)");
@@ -271,11 +360,11 @@ static int launch_flash_tc_p(const CUtensorMap& tmQ, const CUtensorMap& tmK, con
 }
 
 // POLY = column chunks (of 4 per key tile) whose exp2 runs as a polynomial on the FMA pipe (option "fa_poly")
-template <int DQK, int DV>
+template <int DQK, int DV, bool PAGED = false>
 static int launch_flash_tc(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const FaParams& p,
                            dim3 grid, cudaStream_t st) {
-    if (p.poly_chunks >= 1) return launch_flash_tc_p<DQK, DV, 1>(tmQ, tmK, tmV, p, grid, st);
-    return launch_flash_tc_p<DQK, DV, 0>(tmQ, tmK, tmV, p, grid, st);
+    if (p.poly_chunks >= 1) return launch_flash_tc_p<DQK, DV, 1, PAGED>(tmQ, tmK, tmV, p, grid, st);
+    return launch_flash_tc_p<DQK, DV, 0, PAGED>(tmQ, tmK, tmV, p, grid, st);
 }
 
 // 4-D view (D, tokens, heads, batch) of a strided activation; box = 64 columns x 128 tokens, 128B swizzle
@@ -347,4 +436,53 @@ extern "C" int vita_attention_fwd(const void* q, const void* k, const void* v, v
         return flash_tc_dispatch<128, 64>(q, k, v, q_strides, k_strides, v_strides, p, Bi, Hq, Hkv, st);
     set_last_error("vita_attention_fwd: unsupported head dims (supported: 128/128, 64/64, 128/64)");
     return VITA_ERR_INVALID;
+}
+
+extern "C" int vita_attention_prefill_paged(const void* q, int64_t q_token_stride, const void* k_cache,
+                                            const void* v_cache, int64_t n_slots, const int32_t* block_table,
+                                            int64_t bt_stride, const int32_t* query_start_loc, const int32_t* ctx_lens,
+                                            const int32_t* tiles, int64_t n_tiles, void* out, int64_t o_token_stride,
+                                            int64_t T, int64_t n_q_heads, int64_t n_kv_heads, int64_t head_dim,
+                                            int64_t page_size, float scale, void* stream) {
+    VITA_REQUIRE(head_dim == 128, "head_dim must be 128 (Mixtral GQA)");
+    VITA_REQUIRE(page_size == 16 || page_size == 32 || page_size == 64 || page_size == 128,
+                 "page_size must be 16, 32, 64 or 128");
+    VITA_REQUIRE(n_kv_heads > 0 && n_q_heads % n_kv_heads == 0, "n_q_heads must be a multiple of n_kv_heads");
+    VITA_REQUIRE(n_q_heads <= 65535, "head count exceeds the grid limit");
+    VITA_REQUIRE(aligned16(q) && aligned16(k_cache) && aligned16(v_cache) && aligned16(out),
+                 "q / caches / out must be 16-byte aligned");
+    VITA_REQUIRE(q_token_stride % 8 == 0 && o_token_stride % 8 == 0 && q_token_stride >= n_q_heads * head_dim &&
+                     o_token_stride >= n_q_heads * head_dim,
+                 "token strides must cover the q heads and keep 16-byte row alignment");
+    VITA_REQUIRE(scale > 0.0f, "softmax scale must be positive");
+    VITA_REQUIRE(n_tiles >= 0 && n_tiles <= 0x7fffffff && T >= 0 && n_slots > 0 && bt_stride > 0,
+                 "bad tile count, token count, slot count or block-table stride");
+    if (n_tiles == 0 || T == 0) return VITA_OK;
+    VITA_REQUIRE(block_table && query_start_loc && ctx_lens && tiles, "null block_table / query_start_loc / ctx_lens / tiles");
+    FaParams p{};
+    p.o = static_cast<__nv_bfloat16*>(out);
+    p.o_ts = o_token_stride;
+    p.o_hs = head_dim;
+    p.group = static_cast<int>(n_q_heads / n_kv_heads);
+    p.causal = 1;
+    p.scale_log2 = scale * 1.4426950408889634f;
+    p.poly_chunks = option("fa_poly");
+    p.tiles = tiles;
+    p.qsl = query_start_loc;
+    p.ctx = ctx_lens;
+    p.block_table = block_table;
+    p.bt_stride = static_cast<int>(bt_stride);
+    p.page_shift = page_size == 16 ? 4 : page_size == 32 ? 5 : page_size == 64 ? 6 : 7;
+    CUtensorMap tmQ, tmK, tmV;
+    int rc = make_qkv_map(&tmQ, q, 128, T, n_q_heads, 1, q_token_stride, head_dim, 0);
+    if (rc) return rc;
+    const uint64_t dims[3] = {128, static_cast<uint64_t>(n_kv_heads), static_cast<uint64_t>(n_slots)};
+    const uint64_t strides[2] = {128 * 2, static_cast<uint64_t>(n_kv_heads) * 128 * 2};
+    const uint32_t box[3] = {64, 1, static_cast<uint32_t>(page_size)};
+    rc = make_tensor_map_bf16(&tmK, k_cache, 3, dims, strides, box, true);
+    if (rc) return rc;
+    rc = make_tensor_map_bf16(&tmV, v_cache, 3, dims, strides, box, true);
+    if (rc) return rc;
+    const dim3 grid(static_cast<unsigned>(n_tiles), static_cast<unsigned>(n_q_heads), 1);
+    return launch_flash_tc<128, 128, true>(tmQ, tmK, tmV, p, grid, static_cast<cudaStream_t>(stream));
 }

@@ -22,8 +22,17 @@ every query of a session and the hand-off is bookkeeping:
   * interrupt hand-off -- a query whose first token is NOT negative interrupts the running answer of the same session
     (`other_stop_event.set()`, :340-353): the older request is retired at that step with the tokens it has produced.
 
-`ContinuousBatcher` only talks to an `engine` object (prefill / step / swap / read_tokens / reset_slot / first_token), so
-the policy is unit-tested on the CPU with a deterministic stand-in; `DecoderEngine` binds it to `VITAMixtralForCausalLM`.
+Chunked admission (`prefill_chunk`, a per-step token budget like vLLM's `max_num_batched_tokens`): a long arriving
+prompt would otherwise stall every running stream for its whole prefill.  With a budget, the arriving request's
+encoders and splice run once (`begin_prefill`), then its rows are prefilled in chunks of at most `prefill_chunk`
+tokens (`prefill_rows`), one chunk per step, each followed by the decode step of the running prefix.  One request at a
+time is admitted this way; it sits in slot n_active, right behind the prefix, and moves down with it when a running
+request retires.  Its duplex events are decided after the final chunk, when its first token is known.  With nothing
+running the whole prompt goes in at once.
+
+`ContinuousBatcher` only talks to an `engine` object (prefill / step / swap / read_tokens / reset_slot / first_token, and
+begin_prefill / prefill_rows for chunked admission), so the policy is unit-tested on the CPU with a deterministic
+stand-in; `DecoderEngine` binds it to `VITAMixtralForCausalLM`.
 """
 from __future__ import annotations
 
@@ -63,9 +72,12 @@ def swap_rows(tensors: Sequence[torch.Tensor], i: int, j: int) -> None:
 
 
 class ContinuousBatcher:
-    def __init__(self, engine, max_batch: int, sync_every: int = 1):
-        assert max_batch >= 1 and sync_every >= 1
+    def __init__(self, engine, max_batch: int, sync_every: int = 1, prefill_chunk: Optional[int] = None):
+        """`prefill_chunk`: prompt tokens a step may prefill while other requests are running (None: arrivals are
+        prefilled whole before the next decode step)."""
+        assert max_batch >= 1 and sync_every >= 1 and (prefill_chunk is None or prefill_chunk >= 1)
         self.engine, self.max_batch, self.sync_every = engine, max_batch, sync_every
+        self.prefill_chunk = prefill_chunk
 
     def run(self, requests: Sequence[Request], on_step: Optional[Callable[[int, int], None]] = None) -> Dict[int, List[int]]:
         """Runs every request to completion; returns {rid: generated tokens (cut after EOS / max_new_tokens)}.
@@ -75,35 +87,25 @@ class ContinuousBatcher:
         done: Dict[int, List[int]] = {}
         step = 0
         since_sync = 0
-        while pending or active:
-            while pending and pending[0].arrival_step <= step and len(active) < self.max_batch:
+        adm = None                          # chunked admission in progress: [request, prompt rows, rows prefilled]
+        while pending or active or adm is not None:
+            while adm is None and pending and pending[0].arrival_step <= step and len(active) < self.max_batch:
                 r = pending.pop(0)
                 slot = len(active)
                 self.engine.reset_slot(slot)
-                self.engine.prefill(slot, r)
-                r.admitted_step, r.steps = step, 0
-                if r.negative_token_id is not None or r.session is not None:
-                    first = self.engine.first_token(slot)            # the state token: known right after the prefill
-                    if r.negative_token_id is not None and first == r.negative_token_id:
-                        # negative audio: never enters the decode batch (the slot is simply reused by the next arrival)
-                        r.tokens, r.finished_step, r.outcome = [first], step, "negative"
-                        done[r.rid] = r.tokens
-                        continue
-                    if r.session is not None:                        # a real query: interrupt the running answer
-                        for old_slot in sorted((i for i, o in enumerate(active) if o.session == r.session),
-                                               reverse=True):
-                            old = active[old_slot]
-                            old.tokens = self.engine.read_tokens(old_slot)[: min(old.steps, old.max_new_tokens)]
-                            old.finished_step, old.outcome = step, "interrupted"
-                            done[old.rid] = old.tokens
-                            last = len(active) - 1
-                            # the new request sits in slot len(active) (not yet appended): move it down with the rest
-                            if old_slot != last:
-                                self.engine.swap(old_slot, last)
-                                active[old_slot] = active[last]
-                            active.pop()
-                            self.engine.swap(last, last + 1)          # keep the new request right behind the prefix
-                active.append(r)
+                if self.prefill_chunk is None:
+                    self.engine.prefill(slot, r)
+                    self._enter(r, active, done, step)
+                else:
+                    adm = [r, self.engine.begin_prefill(slot, r), 0]
+            if adm is not None:
+                r, S, s0 = adm
+                n = min(self.prefill_chunk, S - s0) if active else S - s0   # nobody waiting: the rest at once
+                self.engine.prefill_rows(len(active), s0, n, s0 + n == S)
+                adm[2] = s0 + n
+                if adm[2] == S:
+                    adm = None
+                    self._enter(r, active, done, step)
             if not active:
                 if not pending:
                     break                           # the last arrivals were dropped as negative queries
@@ -119,10 +121,36 @@ class ContinuousBatcher:
             budget_hit = any(r.steps >= r.max_new_tokens for r in active)
             if since_sync >= self.sync_every or budget_hit:
                 since_sync = 0
-                self._retire(active, done, step)
+                self._retire(active, done, step, adm is not None)
         return done
 
-    def _retire(self, active: List[Request], done: Dict[int, List[int]], step: int) -> None:
+    def _enter(self, r: Request, active: List[Request], done: Dict[int, List[int]], step: int) -> None:
+        """The prompt of `r` (in slot len(active)) is prefilled: decide its duplex events, then join the decode batch."""
+        slot = len(active)
+        r.admitted_step, r.steps = step, 0
+        if r.negative_token_id is not None or r.session is not None:
+            first = self.engine.first_token(slot)            # the state token: known right after the prefill
+            if r.negative_token_id is not None and first == r.negative_token_id:
+                # negative audio: never enters the decode batch (the slot is simply reused by the next arrival)
+                r.tokens, r.finished_step, r.outcome = [first], step, "negative"
+                done[r.rid] = r.tokens
+                return
+            if r.session is not None:                        # a real query: interrupt the running answer
+                for old_slot in sorted((i for i, o in enumerate(active) if o.session == r.session), reverse=True):
+                    old = active[old_slot]
+                    old.tokens = self.engine.read_tokens(old_slot)[: min(old.steps, old.max_new_tokens)]
+                    old.finished_step, old.outcome = step, "interrupted"
+                    done[old.rid] = old.tokens
+                    last = len(active) - 1
+                    # the new request sits in slot len(active) (not yet appended): move it down with the rest
+                    if old_slot != last:
+                        self.engine.swap(old_slot, last)
+                        active[old_slot] = active[last]
+                    active.pop()
+                    self.engine.swap(last, last + 1)          # keep the new request right behind the prefix
+        active.append(r)
+
+    def _retire(self, active: List[Request], done: Dict[int, List[int]], step: int, admitting: bool = False) -> None:
         finished = []
         for slot, r in enumerate(active):
             toks = self.engine.read_tokens(slot)[: r.steps]
@@ -141,6 +169,8 @@ class ContinuousBatcher:
                 self.engine.swap(slot, last)
                 active[slot] = active[last]
             active.pop()
+            if admitting:                               # the request being admitted stays right behind the prefix
+                self.engine.swap(last, last + 1)
 
 
 class DecoderEngine:
@@ -153,6 +183,7 @@ class DecoderEngine:
         the batched GEMM step (faster; the two paths round differently, so tokens are no longer batch-invariant)."""
         self.model, self.llm, self.use_graph, self.overrun = model, model.llm, use_graph, overrun
         self.lone_fast_path = lone_fast_path
+        self._adm = None                    # (prompt rows, sampled) of the request being admitted in chunks
         c = self.llm.cache
         self._slot_tensors = [c.block_table, c.slot_map, c.cache_len, c.cur_pos, self.llm.best, self.llm.token_log,
                               self.llm.gen_count, *self.llm.sampling.tensors]
@@ -166,12 +197,32 @@ class DecoderEngine:
     def prefill(self, slot: int, request: Request) -> None:
         p = request.payload
         emb, lens = self.model._embeds_for(p["input_ids"], p.get("images"), p.get("audios"))
-        need = int(lens[0]) + request.max_new_tokens + self.overrun
+        self._check(request, int(lens[0]))
+        self.llm.sampling.set(slot, request.sampling)
+        self.llm.prefill(emb[0, : lens[0]].contiguous(), slot=slot, sampled=request.sampling is not None)
+
+    def begin_prefill(self, slot: int, request: Request) -> int:
+        """Chunked admission: run the encoders and the splice once, keep the prompt rows; returns their count."""
+        p = request.payload
+        emb, lens = self.model._embeds_for(p["input_ids"], p.get("images"), p.get("audios"))
+        S = int(lens[0])
+        self._check(request, S)
+        self.llm.sampling.set(slot, request.sampling)
+        self._adm = (emb[0, :S].contiguous(), request.sampling is not None)
+        return S
+
+    def prefill_rows(self, slot: int, start: int, n: int, final: bool) -> None:
+        """Prompt rows [start, start + n) of the request being admitted into `slot` (which holds its first `start`)."""
+        rows, sampled = self._adm
+        self.llm.prefill(rows[start:start + n], slot=slot, sampled=sampled, start=start, final=final)
+        if final:
+            self._adm = None
+
+    def _check(self, request: Request, prompt_len: int) -> None:
+        need = prompt_len + request.max_new_tokens + self.overrun
         if need > self.llm.cache.max_seq_len or request.max_new_tokens > self.llm.max_new_tokens:
             raise ValueError(f"request {request.rid}: {need} KV positions / {request.max_new_tokens} new tokens exceed "
                              f"the engine's capacity ({self.llm.cache.max_seq_len} / {self.llm.max_new_tokens})")
-        self.llm.sampling.set(slot, request.sampling)
-        self.llm.prefill(emb[0, : lens[0]].contiguous(), slot=slot, sampled=request.sampling is not None)
 
     def step(self, n_active: int) -> None:
         # the sampled step when any active request samples (its greedy rows keep the greedy tokens), else the greedy one

@@ -238,21 +238,30 @@ class MixtralDecoder:
 
     @torch.no_grad()
     def prefill(self, inputs_embeds: torch.Tensor, slot: int = 0, all_logits: bool = False,
-                want_last_logits: bool = False, sampled: bool = False, scores: Optional[torch.Tensor] = None):
+                want_last_logits: bool = False, sampled: bool = False, scores: Optional[torch.Tensor] = None,
+                start: int = 0, final: bool = True):
         """One sequence: inputs_embeds [S, H] bf16 (consumed as the residual stream, modified in place).
 
         Appends S tokens to the KV cache of batch slot `slot` (which must be empty), leaves the arg-max of the last
         position in self.best[slot] (the first generated token) and returns logits [S, V] if `all_logits`.
         `sampled`: the first token is drawn instead (self.sampling's parameters of the slot, counter 0 =
         gen_count[slot] of the empty slot) from the last-row logits; `scores` [rows, V] receives the warped row at
-        row 0."""
+        row 0.
+
+        Chunked prefill / prefix reuse: `start` is the number of tokens the slot already holds (rows get positions
+        start + i and attend the cached ones through the paged-KV attention kernel).  With `final` False the rows are
+        only appended: no LM head, and best / the sampler counter are left alone; the last chunk of a prompt passes
+        `final` True and yields the first token as a whole-prompt prefill does."""
         c, w = self.cfg, self.w
         S, H = inputs_embeds.shape
         assert inputs_embeds.dtype == BF16 and inputs_embeds.is_cuda and inputs_embeds.is_contiguous()
-        if S > self.cache.max_seq_len:
-            raise ValueError(f"prompt of {S} tokens exceeds the KV capacity of {self.cache.max_seq_len} per sequence")
+        if start < 0 or start + S > self.cache.max_seq_len:
+            raise ValueError(f"prompt of {start} + {S} tokens exceeds the KV capacity of {self.cache.max_seq_len} "
+                             f"per sequence")
         if sampled and self.ep_world > 1:
             raise ValueError("sampled decoding is single-GPU: the expert-parallel prefill serves greedy requests")
+        if (start > 0 or not final) and self.ep_world > 1:
+            raise ValueError("chunked prefill is single-GPU: the expert-parallel prefill takes whole prompts")
         if self.ep_mode == "seq":
             return self._prefill_ep_seq(inputs_embeds, slot, all_logits, want_last_logits)
         ws = self._ws(S)
@@ -268,8 +277,11 @@ class MixtralDecoder:
         ids, tw = ws["ids"][:S], ws["tw"][:S]
         perm, rtok, rw = ws["perm"][:2 * S], ws["rtok"][:2 * S], ws["rw"][:2 * S]
         xp, act, yp = ws["xp"][:2 * S], ws["act"][:2 * S], ws["yp"][:2 * S]
-        pos = ws["pos"][:S]
-        slots = self.cache.slot_map[slot, :S]
+        pos = ws["pos"][:S] if start == 0 else torch.arange(start, start + S, dtype=torch.int32, device=self.device)
+        slots = self.cache.slot_map[slot, start:start + S]
+        paged = None
+        if start > 0:
+            paged = ops.PagedPrefill([0, S], [start + S], self.cache.block_table[slot:slot + 1], self.cache.page_size)
         W = c.qkv_rows
         layers = w["layers"]
         fused = self.ep_world == 1 and self.moe_fused
@@ -279,8 +291,11 @@ class MixtralDecoder:
         for li, lw in enumerate(layers):
             # qkv projection, RoPE and the KV append in one kernel (GEMM epilogue)
             ops.linear_qkv_rope(xn, lw["wqkv"], qkv, pos, slots, w["rope"], self.cache.k[li], self.cache.v[li], nq, nkv, D)
-            ops.attention(qkv, qkv[:, nq * D:], qkv[:, (nq + nkv) * D:], attn, (0, W, D), (0, W, D), (0, W, D),
-                          (0, nq * D, D), 1, nq, nkv, S, S, D, D, None, True, D ** -0.5)
+            if paged is None:
+                ops.attention(qkv, qkv[:, nq * D:], qkv[:, (nq + nkv) * D:], attn, (0, W, D), (0, W, D), (0, W, D),
+                              (0, nq * D, D), 1, nq, nkv, S, S, D, D, None, True, D ** -0.5)
+            else:
+                ops.attention_prefill_paged(qkv, self.cache.k[li], self.cache.v[li], paged, attn, nq, nkv, D, D ** -0.5)
             ops.linear(attn, lw["wo"], residual=h, out=h)
             nxt = layers[li + 1]["ln1"] if li + 1 < len(layers) else (w["norm"] if all_logits else None)
             if fused:
@@ -331,6 +346,8 @@ class MixtralDecoder:
                 dist.all_reduce(ybuf)                                              # NCCL over NVLink (sum, bf16)
                 ops.add_rmsnorm(h, ybuf, nxt, xn if nxt is not None else None, c.rms_norm_eps)
         self.cache.cache_len[slot:slot + 1] += S
+        if not final:
+            return ops.linear(xn, w["lm_head"]) if all_logits else None
         # first generated token: final norm + lm_head + arg-max on the last row only
         self.best[slot:slot + 1].zero_()
         last_logits = self.d_logits[slot:slot + 1] if (want_last_logits or all_logits or sampled) else None

@@ -137,6 +137,55 @@ def attention(q, k, v, out, q_strides, k_strides, v_strides, o_strides, B, n_q, 
     return out
 
 
+class PagedPrefill:
+    """Work list of one step's prompt continuations for attention_prefill_paged, built once per step and reused by
+    every layer.  query_start_loc (B + 1, host): sequence i owns the packed rows [qsl[i], qsl[i + 1]); ctx_lens[i]
+    (host) counts its keys, cached prefix and new rows, all in the pages of block_table[i].  Only the sequences in
+    `seqs` (default: all) are attended; one tile per (sequence, 128-row query block), longest causal rows first."""
+
+    def __init__(self, query_start_loc, ctx_lens, block_table: torch.Tensor, page_size: int, seqs=None):
+        qsl, ctx = [int(x) for x in query_start_loc], [int(x) for x in ctx_lens]
+        B = len(ctx)
+        seqs = list(range(B)) if seqs is None else [int(i) for i in seqs]
+        if len(qsl) != B + 1 or block_table.dim() != 2 or block_table.shape[0] < B:
+            raise _lib.VitaB200Error("PagedPrefill: query_start_loc, ctx_lens and block_table rows do not match")
+        _chk(block_table, torch.int32, "block_table", contiguous=False)
+        if block_table.stride(1) != 1:
+            raise _lib.VitaB200Error("PagedPrefill: block_table rows must be contiguous")
+        tiles = []
+        for i in seqs:
+            c, n = qsl[i + 1] - qsl[i], ctx[i]
+            if not 0 < c <= n or qsl[i] < 0 or qsl[i + 1] > qsl[-1]:
+                raise _lib.VitaB200Error(f"PagedPrefill: sequence {i} has {c} new rows and a context of {n}")
+            if (n + page_size - 1) // page_size > block_table.shape[1]:
+                raise _lib.VitaB200Error(f"PagedPrefill: a context of {n} needs more than {block_table.shape[1]} pages")
+            tiles += [(n - c + 128 * b, i, b) for b in range((c + 127) // 128)]
+        tiles.sort(key=lambda t: -t[0])
+        self.T, self.page_size, self.block_table, self.n_tiles = qsl[-1], int(page_size), block_table, len(tiles)
+        buf = torch.tensor([x for t in tiles for x in t[1:]] + qsl + ctx, dtype=torch.int32).to(block_table.device)
+        n = 2 * len(tiles)
+        self.tiles, self.qsl, self.ctx = buf[:n], buf[n:n + B + 1], buf[n + B + 1:]
+
+
+def attention_prefill_paged(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, plan: PagedPrefill,
+                            out: torch.Tensor, n_q: int, n_kv: int, head_dim: int, scale: float) -> torch.Tensor:
+    """Causal attention of prompt continuations over the paged cache (include/vita_b200.h).  q [T, >= n_q * head_dim]
+    (rows may be strided, e.g. the packed qkv), k/v_cache [slots, n_kv, head_dim], out [T, n_q * head_dim] (rows may
+    be strided); row r of sequence i attends its keys <= ctx_lens[i] - (qsl[i + 1] - qsl[i]) + r.  Rows of sequences
+    outside the plan are left as they are."""
+    _chk(q, BF16, "q", contiguous=False); _chk(out, BF16, "out", contiguous=False)
+    _chk(k_cache, BF16, "k_cache"); _chk(v_cache, BF16, "v_cache")
+    if q.shape[0] != plan.T or out.shape[0] != plan.T or q.stride(1) != 1 or out.stride(1) != 1 \
+            or out.shape[1] < n_q * head_dim or k_cache.shape != v_cache.shape or k_cache.dim() != 3 \
+            or tuple(k_cache.shape[1:]) != (n_kv, head_dim):
+        raise _lib.VitaB200Error("attention_prefill_paged: shape mismatch")
+    bt = plan.block_table
+    _lib.call("vita_attention_prefill_paged", _p(q), q.stride(0), _p(k_cache), _p(v_cache), k_cache.shape[0], _p(bt),
+              bt.stride(0), _p(plan.qsl), _p(plan.ctx), _p(plan.tiles), plan.n_tiles, _p(out), out.stride(0), plan.T,
+              n_q, n_kv, head_dim, plan.page_size, float(scale), _stream())
+    return out
+
+
 def decode_attention_workspace(B: int, n_kv: int, splits: int, device) -> torch.Tensor:
     n = _lib.load().vita_decode_attention_workspace_bytes(B, n_kv, splits)
     return torch.zeros(n, dtype=torch.uint8, device=device)

@@ -9,8 +9,9 @@ What the engine hands the model per step is captured by `TokenBatch` (the fields
 slot mapping, block tables, sequence / query lengths); the engine's block tables and KV tensors are used as they are --
 `kv_caches[l]` is vLLM's flash layout [2, num_blocks, block_size, n_kv_heads, head_dim], which is exactly the layout
 `vita_gemm_qkv_rope` / `vita_decode_attention` address (page = block).  A step may mix fresh prompts (attention over the
-prompt itself, FlashAttention kernel) and single-token decodes (paged decode kernel); chunked prefill / prefix caching
-(a prompt continuing cached pages) is not supported and raises.
+prompt itself, FlashAttention kernel), single-token decodes (paged decode kernel) and multi-token continuations of
+cached pages -- chunked-prefill chunks and prompts whose prefix the engine found in its prefix cache -- which take the
+paged-KV FlashAttention kernel, all of them in one launch per layer.
 
 The reference class was written against vLLM 0.5.5, whose model API no longer exists in the installed 0.22 (probed,
 SURVEY.md section 8b).  `register()` registers this class under the reference's architecture name with the installed
@@ -176,15 +177,18 @@ class MixtralForConditionalGeneration:
         W_ = c.qkv_rows
         qsl, seq_lens = list(meta.query_start_loc), list(meta.seq_lens)
         assert qsl[-1] == T and len(seq_lens) == len(qsl) - 1
-        prefills, decodes = [], []
+        prefills, conts, decodes = [], [], []
         for i, sl in enumerate(seq_lens):
             n = qsl[i + 1] - qsl[i]
             if n == sl:
                 prefills.append((qsl[i], n))
             elif n == 1:
                 decodes.append(i)
+            elif 1 < n < sl:                                # chunked prefill / prefix caching: continues cached pages
+                conts.append(i)
             else:
-                raise NotImplementedError("chunked prefill / prefix caching: a multi-token query over cached pages")
+                raise ValueError(f"sequence {i}: {n} query tokens for a context of {sl}")
+        paged = ops.PagedPrefill(qsl, seq_lens, meta.block_tables, self.block_size, conts) if conts else None
         if decodes:
             d0 = qsl[decodes[0]]
             assert [qsl[i] for i in decodes] == list(range(d0, d0 + len(decodes))), "decode tokens must be contiguous"
@@ -209,6 +213,8 @@ class MixtralForConditionalGeneration:
                 q = qkv[r0:r0 + n]
                 ops.attention(q, q[:, nq * D:], q[:, (nq + nkv) * D:], attn[r0:r0 + n], (0, W_, D), (0, W_, D),
                               (0, W_, D), (0, nq * D, D), 1, nq, nkv, n, n, D, D, None, True, D ** -0.5)
+            if paged is not None:
+                ops.attention_prefill_paged(qkv, kc, vc, paged, attn, nq, nkv, D, D ** -0.5)
             if decodes:
                 ops.decode_attention(qkv[d0:d0 + nd], kc, vc, bt_dec, cur_dec, attn[d0:d0 + nd], self._dec_ws[nd], nq,
                                      nkv, D, self.block_size, llm.decode_splits, D ** -0.5, q_stride=W_)
