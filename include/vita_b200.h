@@ -187,11 +187,6 @@ int vita_ep_reduce_norm_gather(const void* rs_buf, const int32_t* my_flags, void
 int vita_ep_push(void* const* peer_base, const int64_t* offsets, const int64_t* bytes, int64_t n_ranges,
                  int64_t n_ranks, int64_t my_rank, void* stream);
 
-/* expert-parallel tail of a decoder layer (NCCL variant): h += y where y is the all-reduced sum of the ranks' partial MoE outputs
- * (each rank ran vita_moe_combine on a zeroed buffer with only its local experts' rows filled); optional next RMSNorm. */
-int vita_add_rmsnorm(void* h, const void* y, const void* next_norm_w, void* xn_out, int64_t n_tok, int64_t H, float eps,
-                     void* stream);
-
 /* ---- InternViT front / back end --------------------------------------------------------------------------- */
 /* im2col for Conv2d(3,1024,k=14,s=14) (modeling_intern_vit.py:80-85,109): out [n_img*(HW/P)^2, k_pad]. */
 int vita_vit_im2col(const void* images, void* out, int64_t n_img, int64_t C, int64_t HW, int64_t P, int64_t k_pad,

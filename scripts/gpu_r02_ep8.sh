@@ -1,9 +1,9 @@
 #!/bin/bash
-# 8-GPU call: sequence-sharded expert-parallel prefill at full depth: parity at small S + S=4096 timing (32 layers)
+# 8 GPUs: sequence-sharded expert-parallel prefill at full depth: parity at small S + S=4096 timing (32 layers);
+# logs under $OUT (default logs/)
 N=8
-mkdir -p gpurun_out
+OUT=${OUT:-logs}
+mkdir -p "$OUT"
 TR="python -m torch.distributed.run --nnodes=1 --nproc-per-node $N --master-addr 127.0.0.1"
-VITA_B200_EP=seq timeout 600 $TR --master-port 29541 tests/ep_check.py --layers 2 --seq 301 --time-seq 4096 --time-layers 32 > gpurun_out/ep${N}_seq.log 2>&1
-echo "ep_check seq rc=$?" | tee -a gpurun_out/ep${N}_seq.log; grep -E "EP x|mode|Error" gpurun_out/ep${N}_seq.log | tail -6 | cut -c1-300
-VITA_B200_EP=p2p timeout 600 $TR --master-port 29542 tests/ep_check.py --layers 2 --seq 301 --time-seq 4096 --time-layers 32 > gpurun_out/ep${N}_p2p.log 2>&1
-echo "ep_check p2p rc=$?" | tee -a gpurun_out/ep${N}_p2p.log; grep -E "EP x|mode|Error" gpurun_out/ep${N}_p2p.log | tail -6 | cut -c1-300
+timeout 600 $TR --master-port 29541 tests/ep_check.py --layers 2 --seq 301 --time-seq 4096 --time-layers 32 > $OUT/ep${N}.log 2>&1
+echo "ep_check rc=$?" | tee -a $OUT/ep${N}.log; grep -E "EP x|bit-identical|Error" $OUT/ep${N}.log | tail -6 | cut -c1-300

@@ -32,20 +32,18 @@ def main():
     dec = MixtralDecoder(cfg.llm, ep_w, dev, max_seq_len=args.seq + 64, max_new_tokens=8)
     g = torch.Generator(device=dev).manual_seed(11)
     emb = (torch.randn(args.seq, cfg.llm.hidden_size, device=dev, generator=g) * 0.05).to(torch.bfloat16)
-    mode = dec.ep_mode
     logits_ep = dec.prefill(emb.clone(), slot=0, all_logits=True).float()
     tok_ep = int(0xFFFFFFFF - (int(dec.best[0]) & 0xFFFFFFFF))
-    if mode == "seq":
-        # every rank returns the logits of its own token chunk, the owner of the last token holds the arg-max
-        chunk = dec.ep_chunk(args.seq)
-        pad = torch.zeros(chunk, logits_ep.shape[1], device=dev)
-        pad[: logits_ep.shape[0]] = logits_ep
-        parts = [torch.empty_like(pad) for _ in range(world)]
-        dist.all_gather(parts, pad)
-        logits_ep = torch.cat(parts)[: args.seq]
-        t = torch.tensor([tok_ep if dec.best[0] != 0 else -1], device=dev)
-        dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        tok_ep = int(t)
+    # every rank returns the logits of its own token chunk, the owner of the last token holds the arg-max
+    chunk = dec.ep_chunk(args.seq)
+    pad = torch.zeros(chunk, logits_ep.shape[1], device=dev)
+    pad[: logits_ep.shape[0]] = logits_ep
+    parts = [torch.empty_like(pad) for _ in range(world)]
+    dist.all_gather(parts, pad)
+    logits_ep = torch.cat(parts)[: args.seq]
+    t = torch.tensor([tok_ep if dec.best[0] != 0 else -1], device=dev)
+    dist.all_reduce(t, op=dist.ReduceOp.MAX)
+    tok_ep = int(t)
     ok = True
     if rank == 0:
         full_w = W.random_packed(cfg, dev, seed=3, parts=("llm",))["llm"]
@@ -53,21 +51,11 @@ def main():
         logits_1 = ref.prefill(emb.clone(), slot=0, all_logits=True).float()
         tok_1 = int(0xFFFFFFFF - (int(ref.best[0]) & 0xFFFFFFFF))
         row_err = (logits_ep - logits_1).abs().amax(-1) / logits_1.abs().max()
-        # identical routing on both sides (same kernels, same inputs); only the order of the bf16 partial sums differs
         print(f"EP x{world} vs single GPU: median row err {row_err.median():.3e}, max {row_err.max():.3e}; "
               f"first token {tok_ep} vs {tok_1}")
-        if mode in ("seq", "p2p"):
-            # product modes: every (token, k) row is produced once and summed in the single-GPU order -> bit-identical
-            ok = bool(torch.equal(logits_ep, logits_1)) and tok_ep == tok_1
-            print(f"mode {mode}: bit-identical logits: {bool(torch.equal(logits_ep, logits_1))}")
-        else:
-            # library baseline (bf16 partial sums through an NCCL all-reduce): every row is rounded differently from the
-            # single-GPU model, so a token whose next router decision is a near-tie takes another expert and ITS row is
-            # off by what a replaced expert explains (DESIGN.md section 1: chaos of a random-init MoE) -- a bound on the
-            # bulk of the rows is all this variant can promise; the product modes above are held to bit equality
-            frac_ok = float((row_err < 4e-2).float().mean())
-            print(f"mode nccl: rows < 4e-2: {frac_ok:.4f}, 95th percentile {float(row_err.quantile(0.95)):.3e}")
-            ok = bool(row_err.median() < 1e-2) and frac_ok > 0.93
+        # every (token, k) row is produced once and summed in the single-GPU order -> bit-identical
+        ok = bool(torch.equal(logits_ep, logits_1)) and tok_ep == tok_1
+        print(f"bit-identical logits: {bool(torch.equal(logits_ep, logits_1))}")
         del ref, full_w
     if args.time_seq:
         cfg_t = VitaConfig.full(args.time_layers)

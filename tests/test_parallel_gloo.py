@@ -54,8 +54,10 @@ def test_single_process_degenerates():
 
 
 def _ep_worker(rank, world, port, q):
-    """Expert-parallel decomposition of the MoE block: sum over ranks of the local experts' weighted outputs
-    (what MixtralDecoder.prefill all-reduces) equals the full MixtralSparseMoeBlock of the oracle."""
+    """Expert-parallel decomposition of the MoE block: the ranks' expert ranges (weights.expert_range) split the
+    experts so that the sum over ranks of the local experts' weighted outputs equals the full MixtralSparseMoeBlock of
+    the oracle.  (The expert-parallel prefill sums these rows at each token's owning rank; an all-reduce here stands
+    for that exchange.)"""
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), WORLD_SIZE=str(world), RANK=str(rank),
                       LOCAL_RANK=str(rank))
     import torch.nn.functional as F

@@ -120,3 +120,43 @@ def test_placeholder_count_mismatch_raises(golden):
                                       None, IMG_ID)
     with pytest.raises(ValueError, match="expected shape"):   # mixtral.py:974-979
         m._validate_pixel_values(torch.zeros(1, 3, 8, 8))
+
+
+def test_adapter_equals_decoder_bitwise():
+    """The adapter runs the decoder's layer loop over the engine's pages: the same kernels over the same rows.  One
+    whole prompt gives the logits of `prefill(all_logits=True)`, and a decode step of two sequences (over a copy of the
+    decoder's pages) the `d_logits` of `decode_step_batched`, bit for bit."""
+    from vita_b200.model.mixtral import MixtralDecoder
+    from vita_b200.vllm_adapter import MixtralForConditionalGeneration, TokenBatch
+    cfg = VitaConfig.tiny()
+    c, dev = cfg.llm, torch.device("cuda")
+    packed = W.pack(W.synthetic_state(cfg, 0), cfg, dev)
+    m = MixtralForConditionalGeneration(cfg, device=dev, packed=packed)
+    llm = MixtralDecoder(c, packed["llm"], dev, max_batch=2, max_seq_len=128, max_new_tokens=8)
+    cache, bs = llm.cache, llm.cache.page_size
+    g = torch.Generator().manual_seed(6)
+    prompts = [torch.randint(3, 1900, (n,), generator=g).tolist() for n in (37, 20)]
+    embeds = lambda ids: packed["llm"]["embed"][torch.tensor(ids, device=dev)]
+
+    # one whole prompt, all rows scored
+    p = prompts[0]
+    S = len(p)
+    want = llm.prefill(embeds(p), slot=0, all_logits=True)
+    kv = [torch.zeros(2, k.shape[0] // bs, bs, c.num_key_value_heads, c.head_dim, dtype=k.dtype, device=dev)
+          for k in cache.k]
+    meta = TokenBatch(cache.slot_map[0, :S].contiguous(), cache.block_table[:1], [0, S], [S])
+    got = m.compute_logits(m.forward(torch.tensor(p), torch.arange(S), kv, meta))
+    assert torch.equal(got, want), f"{int((got != want).any(-1).sum())} of {S} prompt logits rows differ"
+
+    # one decode step of two sequences
+    llm.reset()
+    for b, p in enumerate(prompts):
+        llm.prefill(embeds(p), slot=b)
+    kv = [torch.stack([k, v]).view(2, -1, bs, c.num_key_value_heads, c.head_dim) for k, v in zip(cache.k, cache.v)]
+    toks = (0xFFFFFFFF - (llm.best[:2] & 0xFFFFFFFF)).tolist()
+    lens = [len(p) for p in prompts]
+    meta = TokenBatch(torch.stack([cache.slot_map[b, n] for b, n in enumerate(lens)]), cache.block_table[:2], [0, 1, 2],
+                      [n + 1 for n in lens])
+    got = m.compute_logits(m.forward(torch.tensor(toks), torch.tensor(lens), kv, meta))
+    llm.decode_step_batched(2, use_graph=False)
+    assert torch.equal(got, llm.d_logits[:2]), "decode-step logits differ"

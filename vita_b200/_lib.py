@@ -50,7 +50,6 @@ SIGNATURES = {
     "vita_moe_route_scatter": (c_int, [P, P, P, P, P, P, P, P, P, I64, I64, I64, I64, c_float, P]),
     "vita_moe_gemm_gate_up_silu_slots": (c_int, [P, P, P, P, I64, I64, I64, I64, I64, P]),
     "vita_moe_gemm_down_slots": (c_int, [P, P, P, P, P, I64, I64, I64, I64, I64, P]),
-    "vita_add_rmsnorm": (c_int, [P, P, P, P, I64, I64, c_float, P]),
     "vita_vit_im2col": (c_int, [P, P, I64, I64, I64, I64, I64, P]),
     "vita_vit_assemble": (c_int, [P, P, P, P, I64, I64, I64, P]),
     "vita_vit_pixel_shuffle": (c_int, [P, P, I64, I64, I64, c_float, P]),

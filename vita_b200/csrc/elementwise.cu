@@ -564,53 +564,6 @@ moe_combine_kernel(__nv_bfloat16* __restrict__ h, const __nv_bfloat16* __restric
     }
 }
 
-// h += y (expert-parallel: y is the all-reduced MoE output), optionally followed by the next RMSNorm.
-template <int THREADS, int VPT>
-__global__ void __launch_bounds__(THREADS)
-add_rmsnorm_kernel(__nv_bfloat16* __restrict__ h, const __nv_bfloat16* __restrict__ y,
-                   const __nv_bfloat16* __restrict__ next_norm_w, __nv_bfloat16* __restrict__ xn_out, int H, float eps) {
-    __shared__ float red[32];
-    const long long tok = blockIdx.x;
-    const int nvec = H >> 3;
-    uint4* hr = reinterpret_cast<uint4*>(h + tok * H);
-    const uint4* yr = reinterpret_cast<const uint4*>(y + tok * H);
-    uint4 v[VPT];
-    float ss = 0.0f;
-#pragma unroll
-    for (int i = 0; i < VPT; ++i) {
-        const int idx = threadIdx.x + i * THREADS;
-        if (idx < nvec) {
-            float a[8], b[8];
-            unpack8(hr[idx], a);
-            unpack8(yr[idx], b);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) a[j] += b[j];
-            v[i] = pack8(a);
-            hr[idx] = v[i];
-            unpack8(v[i], a);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) ss += a[j] * a[j];
-        }
-    }
-    if (next_norm_w == nullptr) return;
-    const float tot = block_sum<THREADS>(ss, red);
-    const float inv = rsqrtf(tot / static_cast<float>(H) + eps);
-    const uint4* wr = reinterpret_cast<const uint4*>(next_norm_w);
-    uint4* xr = reinterpret_cast<uint4*>(xn_out + tok * H);
-#pragma unroll
-    for (int i = 0; i < VPT; ++i) {
-        const int idx = threadIdx.x + i * THREADS;
-        if (idx < nvec) {
-            float f[8], g[8];
-            unpack8(v[i], f);
-            unpack8(__ldg(wr + idx), g);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] = f[j] * inv * g[j];
-            xr[idx] = pack8(f);
-        }
-    }
-}
-
 // ------------------------------------------------------------------------------------------------ expert-parallel tail
 // Flags live in symmetric memory: flags[which][src_rank] of every rank is written by src_rank with a monotonically
 // increasing epoch (st.release.sys after a system fence), waited for with ld.acquire.sys.
@@ -1051,15 +1004,6 @@ extern "C" int vita_ep_reduce_norm_gather(const void* rs_buf, const int32_t* my_
         reinterpret_cast<__nv_bfloat16* const*>(peer_xn), BF(next_norm_w), (int)tok0, (int)n_ranks, (int)my_rank,
         (int)epoch, (int)H, eps, gather ? 1 : 0);
     return check_launch("ep_reduce_norm_gather");
-}
-
-extern "C" int vita_add_rmsnorm(void* h, const void* y, const void* next_norm_w, void* xn_out, int64_t n_tok, int64_t H,
-                                float eps, void* stream) {
-    VITA_REQUIRE(H % 8 == 0 && H <= 8 * 2 * 256, "H must be a multiple of 8 and <= 4096");
-    if (n_tok == 0) return VITA_OK;
-    add_rmsnorm_kernel<256, 2><<<static_cast<unsigned>(n_tok), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        BFM(h), BF(y), BF(next_norm_w), BFM(xn_out), (int)H, eps);
-    return check_launch("add_rmsnorm");
 }
 
 extern "C" int vita_vit_im2col(const void* images, void* out, int64_t n_img, int64_t C, int64_t HW, int64_t P,

@@ -7,7 +7,8 @@ web_demo/vllm_tools/vllm_file/mixtral.py:375-628).  Host code only sequences ker
 from __future__ import annotations
 
 import os
-from typing import List, Optional
+from dataclasses import dataclass
+from typing import Callable, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -51,6 +52,58 @@ class PagedKVCache:
         self.cur_pos.zero_()
 
 
+@dataclass
+class LayerAttention:
+    """The attention kernels every layer runs over the packed qkv rows of one call, chosen once per call.
+    `whole`: (row0, n) prompts that attend only to themselves (causal FlashAttention over the qkv rows);
+    `paged`: the continuations of cached pages (chunked-prefill chunks, prefix-cache hits);
+    `decode`: (row0, n, block_table [n, pages], cur_pos [n], workspace) single-token rows over pages of `page_size`."""
+    whole: Sequence[Tuple[int, int]] = ()
+    paged: Optional[ops.PagedPrefill] = None
+    decode: Optional[tuple] = None
+    page_size: int = 16
+
+    @staticmethod
+    def of_batch(qsl: Sequence[int], seq_lens: Sequence[int], block_tables: torch.Tensor, page_size: int,
+                 decode_workspace: Callable[[int], torch.Tensor]) -> "LayerAttention":
+        """Flattened batch: sequence i owns rows [qsl[i], qsl[i + 1]) and has seq_lens[i] keys including them.  Rows
+        that are the whole context are a prompt, one row is a decode, anything in between continues cached pages.
+        The decode rows must be contiguous; decode_workspace(n) gives the decode-attention workspace of n rows."""
+        whole, conts, decodes = [], [], []
+        for i, sl in enumerate(seq_lens):
+            n = qsl[i + 1] - qsl[i]
+            if n == sl:
+                whole.append((qsl[i], n))
+            elif n == 1:
+                decodes.append(i)
+            elif 1 < n < sl:                                # chunked prefill / prefix caching: continues cached pages
+                conts.append(i)
+            else:
+                raise ValueError(f"sequence {i}: {n} query tokens for a context of {sl}")
+        paged = ops.PagedPrefill(qsl, seq_lens, block_tables, page_size, conts) if conts else None
+        decode = None
+        if decodes:
+            d0, nd = qsl[decodes[0]], len(decodes)
+            assert [qsl[i] for i in decodes] == list(range(d0, d0 + nd)), "decode tokens must be contiguous"
+            cur = torch.tensor([seq_lens[i] - 1 for i in decodes], dtype=torch.int32).to(block_tables.device)
+            decode = (d0, nd, block_tables[decodes].contiguous(), cur, decode_workspace(nd))
+        return LayerAttention(whole, paged, decode, page_size)
+
+    def __call__(self, qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, out: torch.Tensor,
+                 c: LLMConfig, splits: int):
+        nq, nkv, D, W = c.num_attention_heads, c.num_key_value_heads, c.head_dim, c.qkv_rows
+        for r0, n in self.whole:
+            q = qkv[r0:r0 + n]
+            ops.attention(q, q[:, nq * D:], q[:, (nq + nkv) * D:], out[r0:r0 + n], (0, W, D), (0, W, D), (0, W, D),
+                          (0, nq * D, D), 1, nq, nkv, n, n, D, D, None, True, D ** -0.5)
+        if self.paged is not None:
+            ops.attention_prefill_paged(qkv, k_cache, v_cache, self.paged, out, nq, nkv, D, D ** -0.5)
+        if self.decode is not None:
+            r0, n, block_table, cur_pos, workspace = self.decode
+            ops.decode_attention(qkv[r0:r0 + n], k_cache, v_cache, block_table, cur_pos, out[r0:r0 + n], workspace, nq,
+                                 nkv, D, self.page_size, splits, D ** -0.5, q_stride=W)
+
+
 class MixtralDecoder:
     def __init__(self, cfg: LLMConfig, weights: dict, device, max_batch: int = 1, max_seq_len: Optional[int] = None,
                  max_new_tokens: int = 1024, page_size: int = 16, decode_splits: int = 16, shuffle_pages: bool = False):
@@ -65,15 +118,12 @@ class MixtralDecoder:
         if page_rounded > weights["rope"].shape[0]:      # cos/sin table sized from the KV capacity, not a constant
             from ..weights import rope_table
             weights["rope"] = rope_table(page_rounded, cfg.head_dim, cfg.rope_theta).to(self.device)
-        # expert parallelism: this rank holds experts [e_lo, e_hi) of every layer.  Modes (VITA_B200_EP):
-        #   seq  (default) sequence-sharded residual stream: every rank owns S/N tokens for the dense part (qkv, causal
-        #        attention over the all-gathered K/V, o-proj, router); K/V rows and routed activations are all-gathered
-        #        and the expert outputs pushed to the token owners by P2P stores over NVLink symmetric memory
-        #   p2p  replicated dense part, fused P2P combine (kept as the A/B baseline)
-        #   nccl replicated dense part, partial sums + NCCL all-reduce (library baseline)
+        # expert parallelism: this rank holds experts [e_lo, e_hi) of every layer; the residual stream is sequence
+        # sharded: every rank owns S/N tokens for the dense part (qkv, causal attention over the all-gathered K/V,
+        # o-proj, router); K/V rows and routed activations are all-gathered and the expert outputs pushed to the token
+        # owners by P2P stores over NVLink symmetric memory
         self.ep_rank, self.ep_world = weights.get("ep", (0, 1))
-        self.ep_mode = os.environ.get("VITA_B200_EP", "seq") if self.ep_world > 1 else None
-        assert self.ep_mode in (None, "seq", "p2p", "nccl"), "VITA_B200_EP must be seq, p2p or nccl"
+        self.ep_mode = "seq" if self.ep_world > 1 else None
         self.ep_p2p = None
         storage = None
         if self.ep_mode == "seq":
@@ -114,20 +164,16 @@ class MixtralDecoder:
         self.d_slots = torch.zeros(B, dtype=torch.int32, device=dev)
         self._prefill_ws = {}
         # router decisions of every layer (the reference returns them as `router_logits` when asked,
-        # vita_mixtral.py:108,185-190): set to a list to have prefill() and the eager decode step append one
+        # vita_mixtral.py:108,185-190): set to a list to have prefill() and the eager decode steps append one
         # (top-2 ids [T, 2] int32, renormalised weights [T, 2] fp32) pair per layer
         self.route_trace: Optional[list] = None
         # decode: the gate|up kernel can publish the expert pair as soon as its router is done so that the down projection
         # streams its weight rows while gate|up is still running.  Bit-identical; not measured on H100:
         # off unless VITA_B200_EARLY_ROUTE=1
         self.early_route = os.environ.get("VITA_B200_EARLY_ROUTE", "0") == "1"
-        # prefill / batched decode: fused top-2 router + token permute over per-expert slot ranges (0 = align + gather)
-        self.moe_fused = os.environ.get("VITA_B200_MOE_FUSED", "1") == "1"
         per = cfg.num_local_experts // self.ep_world
         self.e_lo, self.e_hi = self.ep_rank * per, (self.ep_rank + 1) * per
         assert weights["layers"][0]["w13"].shape[0] == per, "expert tensors do not match the EP layout"
-        if self.ep_mode == "p2p":
-            self._init_ep_p2p()
 
     def _init_ep_seq(self, S_max: int):
         """One NVLink symmetric allocation for the sequence-sharded expert-parallel prefill: receive slots of the
@@ -178,34 +224,6 @@ class MixtralDecoder:
         from ..parallel import sequence_chunk
         return sequence_chunk(S, self.ep_world)
 
-    def _init_ep_p2p(self):
-        """Symmetric (peer-mapped) buffers for the fused expert-parallel combine: every rank can store into every
-        other rank's receive slots, residual stream and normed activations over NVLink."""
-        import torch.distributed as dist
-        import torch.distributed._symmetric_memory as symm_mem
-        c, N, dev = self.cfg, self.ep_world, self.device
-        H, S_max = c.hidden_size, self.cache.max_seq_len
-        chunk_max = (S_max + N - 1) // N
-        al = lambda n: (n + 255) // 256 * 256
-        sizes = [al(chunk_max * 2 * H * 2), al(S_max * H * 2), al(S_max * H * 2), al(2 * N * 4)]
-        offs = [0]
-        for z in sizes:
-            offs.append(offs[-1] + z)
-        sym = symm_mem.empty(offs[-1], dtype=torch.uint8, device=dev)
-        sym.zero_()
-        torch.cuda.synchronize()
-        hdl = symm_mem.rendezvous(sym, dist.group.WORLD)
-        delta = sym.data_ptr() - int(hdl.buffer_ptrs[hdl.rank])      # offset of this tensor inside the allocation
-        bases = [int(p) + delta for p in hdl.buffer_ptrs]
-        assert hdl.world_size == N and hdl.rank == self.ep_rank
-        view = lambda i, dt: sym[offs[i]:offs[i] + sizes[i]].view(dt)
-        ptrs = lambda i: torch.tensor([b + offs[i] for b in bases], dtype=torch.int64, device=dev)
-        self.ep_p2p = dict(
-            sym=sym, hdl=hdl, chunk_max=chunk_max,
-            rs=view(0, BF16), h=view(1, BF16)[:S_max * H].view(S_max, H), xn=view(2, BF16)[:S_max * H].view(S_max, H),
-            flags=view(3, torch.int32), rs_ptrs=ptrs(0), h_ptrs=ptrs(1), xn_ptrs=ptrs(2), flag_ptrs=ptrs(3), epoch=0)
-        dist.barrier()
-
     # ------------------------------------------------------------------------------------------ prefill
     def _ws(self, S: int):
         """Prefill workspaces, grown geometrically and reused."""
@@ -213,7 +231,9 @@ class MixtralDecoder:
         if S > cap:
             c = self.cfg
             cap = max(S, 2 * cap, 128)
-            self._bgraphs = {}    # the batched-step graphs reference the old workspaces
+            # the batched-step graphs reference the old workspaces; cleared in place because a _replay whose warm-up
+            # grows them stores its new graph into this same dict
+            self._bgraphs.clear()
             H, I, E, dev = c.hidden_size, c.intermediate_size, c.num_local_experts, self.device
             with torch.inference_mode(False):      # reused across calls: keep them ordinary tensors
                 self._prefill_ws = self._alloc_ws(cap, H, I, E, dev)
@@ -223,18 +243,49 @@ class MixtralDecoder:
         c = self.cfg
         e = lambda *shape, dt=BF16: torch.empty(*shape, dtype=dt, device=dev)
         # MoE activations in the "slot" layout of the fused router + permute: expert e owns rows [e * cap, (e + 1) * cap)
-        # (any expert may receive every token).  The compact buffers of the align / gather flow (expert parallelism, the
-        # vLLM-shaped adapter) are the first 2 * cap rows of the same storage.
+        # (any expert may receive every token).  The compact buffers of the align / gather flow of expert parallelism
+        # are the first 2 * cap rows of the same storage.
         xs, acts, ys, rws = e(E * cap, H), e(E * cap, I), e(E * cap, H), e(E * cap, dt=torch.float32)
         return dict(
             cap=cap, xn=e(cap, H), qkv=e(cap, c.qkv_rows), attn=e(cap, c.num_attention_heads * c.head_dim),
-            xn2=e(cap, H), ids=e(cap, 2, dt=torch.int32), tw=e(cap, 2, dt=torch.float32),
+            ids=e(cap, 2, dt=torch.int32), tw=e(cap, 2, dt=torch.float32),
             offs=e(E + 1, dt=torch.int32), perm=e(cap * 2, dt=torch.int32), rtok=e(cap * 2, dt=torch.int32),
             xs=xs, acts=acts, ys=ys, rws=rws,
             cnt=torch.zeros(c.num_hidden_layers, E, dtype=torch.int32, device=dev),
-            rw=rws[:cap * 2], xp=xs[:cap * 2], act=acts[:cap * 2], yp=ys[:cap * 2],
-            ybuf=e(cap, H) if self.ep_world > 1 else None, rassign=e(cap * 2, dt=torch.int32),
+            rw=rws[:cap * 2], xp=xs[:cap * 2], act=acts[:cap * 2], rassign=e(cap * 2, dt=torch.int32),
             pos=torch.arange(cap, dtype=torch.int32, device=dev))
+
+    def run_layers(self, h: torch.Tensor, pos: torch.Tensor, slots: torch.Tensor, k_cache: Sequence[torch.Tensor],
+                   v_cache: Sequence[torch.Tensor], attention: LayerAttention, final_norm: bool) -> torch.Tensor:
+        """Every layer over the T rows of the residual stream h [T, H] (updated in place): qkv projection + RoPE at
+        `pos` + K/V append at `slots` of k_cache[l] / v_cache[l], `attention`, o-proj + residual, fused top-2 MoE.
+        Returns xn [T, H] (workspace rows): the final RMSNorm(h) when `final_norm`, not written by the last layer
+        otherwise."""
+        c, w = self.cfg, self.w
+        T = h.shape[0]
+        nq, nkv, D = c.num_attention_heads, c.num_key_value_heads, c.head_dim
+        ws = self._ws(T)
+        xn, qkv, attn, perm = ws["xn"][:T], ws["qkv"][:T], ws["attn"][:T], ws["perm"][:2 * T]
+        tracing = self.route_trace is not None and not torch.cuda.is_current_stream_capturing()
+        ids, tw = (ws["ids"][:T], ws["tw"][:T]) if tracing else (None, None)
+        layers = w["layers"]
+        ws["cnt"].zero_()              # per-layer expert counters of the fused router + permute
+        ops.rmsnorm(h, layers[0]["ln1"], c.rms_norm_eps, out=xn)
+        for li, lw in enumerate(layers):
+            # qkv projection, RoPE and the KV append in one kernel (GEMM epilogue)
+            ops.linear_qkv_rope(xn, lw["wqkv"], qkv, pos, slots, w["rope"], k_cache[li], v_cache[li], nq, nkv, D)
+            attention(qkv, k_cache[li], v_cache[li], attn, c, self.decode_splits)
+            ops.linear(attn, lw["wo"], residual=h, out=h)
+            # router + permute in one kernel (slot layout), grouped GEMMs over the slots, gather-combine
+            cnt = ws["cnt"][li]
+            ops.moe_route_scatter(h, lw["ln2"], lw["gate"], ws["xs"], cnt, perm, ws["rws"], c.rms_norm_eps, ids, tw)
+            if tracing:
+                self.route_trace.append((ids.clone(), tw.clone()))
+            ops.moe_gate_up_slots(ws["xs"], lw["w13"], ws["acts"], cnt, 2 * T)
+            ops.moe_down_slots(ws["acts"], lw["w2"], ws["ys"], cnt, ws["rws"], 2 * T)
+            nxt = layers[li + 1]["ln1"] if li + 1 < len(layers) else (w["norm"] if final_norm else None)
+            ops.moe_combine(h, ws["ys"], perm, nxt, xn if nxt is not None else None, c.rms_norm_eps)
+        return xn
 
     @torch.no_grad()
     def prefill(self, inputs_embeds: torch.Tensor, slot: int = 0, all_logits: bool = False,
@@ -264,87 +315,15 @@ class MixtralDecoder:
             raise ValueError("chunked prefill is single-GPU: the expert-parallel prefill takes whole prompts")
         if self.ep_mode == "seq":
             return self._prefill_ep_seq(inputs_embeds, slot, all_logits, want_last_logits)
-        ws = self._ws(S)
         h = inputs_embeds
-        p2p = self.ep_p2p
-        if p2p is not None:          # the residual stream and the normed activations live in symmetric memory
-            h = p2p["h"][:S]
-            h.copy_(inputs_embeds)
-        nq, nkv, D, E = c.num_attention_heads, c.num_key_value_heads, c.head_dim, c.num_local_experts
-        xn, qkv, attn, xn2 = ws["xn"][:S], ws["qkv"][:S], ws["attn"][:S], ws["xn2"][:S]
-        if p2p is not None:
-            xn = p2p["xn"][:S]
-        ids, tw = ws["ids"][:S], ws["tw"][:S]
-        perm, rtok, rw = ws["perm"][:2 * S], ws["rtok"][:2 * S], ws["rw"][:2 * S]
-        xp, act, yp = ws["xp"][:2 * S], ws["act"][:2 * S], ws["yp"][:2 * S]
-        pos = ws["pos"][:S] if start == 0 else torch.arange(start, start + S, dtype=torch.int32, device=self.device)
-        slots = self.cache.slot_map[slot, start:start + S]
-        paged = None
-        if start > 0:
-            paged = ops.PagedPrefill([0, S], [start + S], self.cache.block_table[slot:slot + 1], self.cache.page_size)
-        W = c.qkv_rows
-        layers = w["layers"]
-        fused = self.ep_world == 1 and self.moe_fused
-        if fused:
-            ws["cnt"].zero_()          # per-layer expert counters of the fused router + permute
-        ops.rmsnorm(h, layers[0]["ln1"], c.rms_norm_eps, out=xn)
-        for li, lw in enumerate(layers):
-            # qkv projection, RoPE and the KV append in one kernel (GEMM epilogue)
-            ops.linear_qkv_rope(xn, lw["wqkv"], qkv, pos, slots, w["rope"], self.cache.k[li], self.cache.v[li], nq, nkv, D)
-            if paged is None:
-                ops.attention(qkv, qkv[:, nq * D:], qkv[:, (nq + nkv) * D:], attn, (0, W, D), (0, W, D), (0, W, D),
-                              (0, nq * D, D), 1, nq, nkv, S, S, D, D, None, True, D ** -0.5)
-            else:
-                ops.attention_prefill_paged(qkv, self.cache.k[li], self.cache.v[li], paged, attn, nq, nkv, D, D ** -0.5)
-            ops.linear(attn, lw["wo"], residual=h, out=h)
-            nxt = layers[li + 1]["ln1"] if li + 1 < len(layers) else (w["norm"] if all_logits else None)
-            if fused:
-                # router + permute in one kernel (slot layout), grouped GEMMs over the slots, gather-combine
-                cnt = ws["cnt"][li]
-                ops.moe_route_scatter(h, lw["ln2"], lw["gate"], ws["xs"], cnt, perm, ws["rws"], c.rms_norm_eps, ids, tw)
-                if self.route_trace is not None:
-                    self.route_trace.append((ids.clone(), tw.clone()))
-                ops.moe_gate_up_slots(ws["xs"], lw["w13"], ws["acts"], cnt, 2 * S)
-                ops.moe_down_slots(ws["acts"], lw["w2"], ws["ys"], cnt, ws["rws"], 2 * S)
-                ops.moe_combine(h, ws["ys"], perm, nxt, xn if nxt is not None else None, c.rms_norm_eps)
-                continue
-            ops.moe_router(h, lw["ln2"], lw["gate"], xn2, ids, tw, c.rms_norm_eps)
-            if self.route_trace is not None:
-                self.route_trace.append((ids.clone(), tw.clone()))
-            ops.moe_align(ids, tw, ws["offs"], perm, rtok, rw, S, E, row_assign=ws["rassign"][:2 * S])
-            ops.row_copy(xn2, rtok, None, xp, 2 * S)
-            if p2p is not None:
-                # fused expert-parallel combine over NVLink peer memory: the down-projection epilogue pushes every
-                # (token, k) row to the token's owner; owners reduce + norm + all-gather by P2P stores
-                N, r = self.ep_world, self.ep_rank
-                chunk = (S + N - 1) // N
-                offs_local = ws["offs"][self.e_lo:]
-                p2p["epoch"] += 1
-                ep = p2p["epoch"]
-                ops.moe_gate_up(xp, lw["w13"], act, offs_local, 2 * S)
-                ops.moe_down_ep(act, lw["w2"], offs_local, rw, ws["rassign"][:2 * S], p2p["rs_ptrs"], 2 * S, chunk)
-                ops.ep_signal(p2p["flag_ptrs"], 0, N, r, ep)
-                n_owned = max(0, min(chunk, S - r * chunk))
-                ops.ep_reduce_norm_gather(p2p["rs"], p2p["flags"], p2p["h_ptrs"], p2p["xn_ptrs"], nxt, r * chunk,
-                                          n_owned, N, r, ep, H, c.rms_norm_eps)
-                ops.ep_signal(p2p["flag_ptrs"], 1, N, r, ep)
-                ops.ep_wait(p2p["flags"], 1, N, ep)
-            elif self.ep_world == 1:
-                ops.moe_gate_up(xp, lw["w13"], act, ws["offs"], 2 * S)
-                ops.moe_down(act, lw["w2"], yp, ws["offs"], rw, 2 * S)
-                ops.moe_combine(h, yp, perm, nxt, xn if nxt is not None else None, c.rms_norm_eps)
-            else:
-                # local experts only: the grouped GEMMs walk offs[e_lo : e_hi + 1]; rows of remote experts stay zero
-                import torch.distributed as dist
-                offs_local = ws["offs"][self.e_lo:]
-                yp.zero_()
-                ops.moe_gate_up(xp, lw["w13"], act, offs_local, 2 * S)
-                ops.moe_down(act, lw["w2"], yp, offs_local, rw, 2 * S)
-                ybuf = ws["ybuf"][:S]
-                ybuf.zero_()
-                ops.moe_combine(ybuf, yp, perm, None, None, c.rms_norm_eps)       # partial sum of the local experts
-                dist.all_reduce(ybuf)                                              # NCCL over NVLink (sum, bf16)
-                ops.add_rmsnorm(h, ybuf, nxt, xn if nxt is not None else None, c.rms_norm_eps)
+        if start == 0:
+            pos, attention = self._ws(S)["pos"][:S], LayerAttention(whole=[(0, S)])
+        else:
+            pos = torch.arange(start, start + S, dtype=torch.int32, device=self.device)
+            plan = ops.PagedPrefill([0, S], [start + S], self.cache.block_table[slot:slot + 1], self.cache.page_size)
+            attention = LayerAttention(paged=plan)
+        xn = self.run_layers(h, pos, self.cache.slot_map[slot, start:start + S], self.cache.k, self.cache.v, attention,
+                             final_norm=all_logits)
         self.cache.cache_len[slot:slot + 1] += S
         if not final:
             return ops.linear(xn, w["lm_head"]) if all_logits else None
@@ -513,77 +492,31 @@ class MixtralDecoder:
 
     @torch.no_grad()
     def decode_step(self, B: int = 1, use_graph: bool = True, want_logits: bool = False, sampled: bool = False):
-        assert self.ep_world == 1, "expert-parallel mode covers the prefill (BASELINE configs[3]); decode is replicated"
-        self._decode_step(B, use_graph, want_logits, sampled)
-
-    def _decode_step(self, B: int = 1, use_graph: bool = True, want_logits: bool = False, sampled: bool = False):
         """Generate one token for batch slots [0, B): consumes self.best, appends to token_log, leaves the next
         arg-max (or, `sampled`, the drawn token) in self.best.  With use_graph the whole step (2 + 5 * layers kernels,
         one more when sampled) replays as one CUDA graph."""
+        assert self.ep_world == 1, "expert-parallel mode covers the prefill (BASELINE configs[3]); decode is replicated"
+        step = lambda: self._decode_step_kernels(B, want_logits, sampled)
         if not use_graph:
-            self._decode_step_kernels(B, want_logits, sampled)
+            step()
             return
         key = (B, want_logits, True) if sampled else (B, want_logits)    # greedy keys keep their (B, want_logits) form
-        if key not in self._graphs:
-            # capture (the kernels were warmed up by an eager step so every cudaFuncSetAttribute already ran)
-            self._snapshot = self._save_state()
-            self._decode_step_kernels(B, want_logits, sampled)
-            torch.cuda.synchronize()
-            self._restore_state(self._snapshot)
-            g = torch.cuda.CUDAGraph()
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                with torch.cuda.graph(g, stream=side):
-                    self._decode_step_kernels(B, want_logits, sampled)
-            torch.cuda.current_stream().wait_stream(side)
-            torch.cuda.synchronize()
-            self._restore_state(self._snapshot)   # capture does not execute, but keep the invariant explicit
-            self._graphs[key] = g
-        self._graphs[key].replay()
+        self._replay(self._graphs, key, step)
 
     # ------------------------------------------------------------------------------------------ batched decode
-    def _batched_step_kernels(self, B: int, want_logits: bool, sampled: bool = False):
+    def _batched_step_kernels(self, B: int, sampled: bool = False):
         """One token for each of B sequences through the GEMM path (weights of every touched expert are streamed once
-        for the whole batch; BASELINE configs[4]).  Same kernels as the prefill, with M = B rows at B different
-        positions, + the paged decode attention."""
+        for the whole batch; BASELINE configs[4]).  The prefill's layer loop with M = B rows at B different
+        positions and the paged decode attention."""
         c, w, cache = self.cfg, self.w, self.cache
-        nq, nkv, D, E, H = c.num_attention_heads, c.num_key_value_heads, c.head_dim, c.num_local_experts, c.hidden_size
-        ws = self._ws(max(B, 16))
         h = self.d_h[:B]
         ops.decode_embed(self.best[:B], self.token_log[:B], self.gen_count[:B], cache.cache_len[:B], cache.cur_pos[:B],
                          w["embed"], h, cache.max_seq_len)
         slots = self.d_slots[:B]
         ops.decode_slots(cache.cur_pos[:B], cache.block_table[:B], slots, cache.page_size)
-        xn, qkv, attn, xn2 = ws["xn"][:B], ws["qkv"][:B], ws["attn"][:B], ws["xn2"][:B]
-        ids, tw = ws["ids"][:B], ws["tw"][:B]
-        perm, rtok, rw = ws["perm"][:2 * B], ws["rtok"][:2 * B], ws["rw"][:2 * B]
-        xp, act, yp = ws["xp"][:2 * B], ws["act"][:2 * B], ws["yp"][:2 * B]
-        layers = w["layers"]
-        if self.moe_fused:
-            ws["cnt"].zero_()
-        ops.rmsnorm(h, layers[0]["ln1"], c.rms_norm_eps, out=xn)
-        for li, lw in enumerate(layers):
-            ops.linear_qkv_rope(xn, lw["wqkv"], qkv, cache.cur_pos[:B], slots, w["rope"], cache.k[li], cache.v[li],
-                                nq, nkv, D)
-            ops.decode_attention(qkv, cache.k[li], cache.v[li], cache.block_table[:B], cache.cur_pos[:B], attn,
-                                 self.attn_ws, nq, nkv, D, cache.page_size, self.decode_splits, D ** -0.5,
-                                 q_stride=c.qkv_rows)
-            ops.linear(attn, lw["wo"], residual=h, out=h)
-            nxt = layers[li + 1]["ln1"] if li + 1 < len(layers) else w["norm"]
-            if self.moe_fused:
-                cnt = ws["cnt"][li]
-                ops.moe_route_scatter(h, lw["ln2"], lw["gate"], ws["xs"], cnt, perm, ws["rws"], c.rms_norm_eps)
-                ops.moe_gate_up_slots(ws["xs"], lw["w13"], ws["acts"], cnt, 2 * B)
-                ops.moe_down_slots(ws["acts"], lw["w2"], ws["ys"], cnt, ws["rws"], 2 * B)
-                ops.moe_combine(h, ws["ys"], perm, nxt, xn, c.rms_norm_eps)
-                continue
-            ops.moe_router(h, lw["ln2"], lw["gate"], xn2, ids, tw, c.rms_norm_eps)
-            ops.moe_align(ids, tw, ws["offs"], perm, rtok, rw, B, E)
-            ops.row_copy(xn2, rtok, None, xp, 2 * B)
-            ops.moe_gate_up(xp, lw["w13"], act, ws["offs"], 2 * B)
-            ops.moe_down(act, lw["w2"], yp, ws["offs"], rw, 2 * B)
-            ops.moe_combine(h, yp, perm, nxt, xn, c.rms_norm_eps)
+        attention = LayerAttention(decode=(0, B, cache.block_table[:B], cache.cur_pos[:B], self.attn_ws),
+                                   page_size=cache.page_size)
+        xn = self.run_layers(h, cache.cur_pos[:B], slots, cache.k, cache.v, attention, final_norm=True)
         logits = ops.linear(xn, w["lm_head"], out=self.d_logits[:B])
         if sampled:          # greedy rows (temperature 0) get argmax_rows' word: a mixed batch keeps their tokens
             self._sample(0, B, None)
@@ -592,18 +525,23 @@ class MixtralDecoder:
 
     @property
     def launches_per_batched_step(self) -> int:
-        return (6 + 8 * self.cfg.num_hidden_layers) if self.moe_fused else (5 + 10 * self.cfg.num_hidden_layers)
+        return 6 + 8 * self.cfg.num_hidden_layers
 
     @torch.no_grad()
     def decode_step_batched(self, B: int, use_graph: bool = True, sampled: bool = False):
         assert self.ep_world == 1 and 1 <= B <= self.max_batch
+        step = lambda: self._batched_step_kernels(B, sampled)
         if not use_graph:
-            self._batched_step_kernels(B, False, sampled)
+            step()
             return
-        key = (B, sampled)
-        if key not in self._bgraphs:           # one captured graph per batch size (continuous batching changes B)
+        self._replay(self._bgraphs, (B, sampled), step)   # one graph per batch size (continuous batching changes B)
+
+    def _replay(self, graphs: dict, key, step):
+        """Replay graphs[key], capturing `step` (a decode step that takes no host input) into it first: an eager
+        warm-up runs every cudaFuncSetAttribute outside the capture, and the decode state it advanced is restored."""
+        if key not in graphs:
             snap = self._save_state()
-            self._batched_step_kernels(B, False, sampled)  # warm-up (cudaFuncSetAttribute etc.)
+            step()
             torch.cuda.synchronize()
             self._restore_state(snap)
             g = torch.cuda.CUDAGraph()
@@ -611,12 +549,12 @@ class MixtralDecoder:
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
                 with torch.cuda.graph(g, stream=side):
-                    self._batched_step_kernels(B, False, sampled)
+                    step()
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
-            self._restore_state(snap)
-            self._bgraphs[key] = g
-        self._bgraphs[key].replay()
+            self._restore_state(snap)   # capture does not execute, but keep the invariant explicit
+            graphs[key] = g
+        graphs[key].replay()
 
     def _save_state(self):
         c = self.cache

@@ -336,12 +336,6 @@ def moe_combine(h, y_perm, perm_row, next_norm_w, xn_out, eps):
               _stream())
 
 
-def add_rmsnorm(h, y, next_norm_w, xn_out, eps):
-    _chk(h, BF16, "h"); _chk(y, BF16, "y")
-    n_tok, H = h.shape
-    _lib.call("vita_add_rmsnorm", _p(h), _p(y), _p(next_norm_w), _p(xn_out), n_tok, H, float(eps), _stream())
-
-
 # ------------------------------------------------------------------------------------------------ InternViT glue
 def vit_im2col(images, out, P, k_pad):
     _chk(images, BF16, "images"); _chk(out, BF16, "out")

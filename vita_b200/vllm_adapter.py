@@ -30,7 +30,7 @@ from . import ops, weights as W
 from .config import VitaConfig
 from .sampling import from_vllm, row_tensors
 from .model.internvit import InternViTVisionTower, VisionProjector
-from .model.mixtral import MixtralDecoder
+from .model.mixtral import LayerAttention, MixtralDecoder
 from .model.whale import AudioEncoder
 
 BF16 = torch.bfloat16
@@ -106,7 +106,7 @@ class MixtralForConditionalGeneration:
     def _bind(self, packed: dict):
         cfg = self.config
         self.packed = packed
-        # the decoder object supplies kernels + workspaces; its own (1-slot) KV cache is unused: the engine owns the KV
+        # the decoder object supplies the layer loop + workspaces; its own (1-slot) KV cache is unused: the engine owns KV
         self.llm = MixtralDecoder(cfg.llm, packed["llm"], self.device, max_batch=1, max_seq_len=64, max_new_tokens=8)
         self.vision_tower = InternViTVisionTower(cfg.vision, packed["vision"], self.device) if "vision" in packed else None
         self.vision_projector = VisionProjector(packed["projector"]) if "projector" in packed else None
@@ -171,62 +171,21 @@ class MixtralForConditionalGeneration:
     __call__ = forward
 
     def _language_model(self, h: torch.Tensor, positions: torch.Tensor, kv_caches, meta: TokenBatch) -> torch.Tensor:
-        llm, c, w = self.llm, self.config.llm, self.packed["llm"]
-        T, H = h.shape
-        nq, nkv, D, E = c.num_attention_heads, c.num_key_value_heads, c.head_dim, c.num_local_experts
-        W_ = c.qkv_rows
+        c = self.config.llm
         qsl, seq_lens = list(meta.query_start_loc), list(meta.seq_lens)
-        assert qsl[-1] == T and len(seq_lens) == len(qsl) - 1
-        prefills, conts, decodes = [], [], []
-        for i, sl in enumerate(seq_lens):
-            n = qsl[i + 1] - qsl[i]
-            if n == sl:
-                prefills.append((qsl[i], n))
-            elif n == 1:
-                decodes.append(i)
-            elif 1 < n < sl:                                # chunked prefill / prefix caching: continues cached pages
-                conts.append(i)
-            else:
-                raise ValueError(f"sequence {i}: {n} query tokens for a context of {sl}")
-        paged = ops.PagedPrefill(qsl, seq_lens, meta.block_tables, self.block_size, conts) if conts else None
-        if decodes:
-            d0 = qsl[decodes[0]]
-            assert [qsl[i] for i in decodes] == list(range(d0, d0 + len(decodes))), "decode tokens must be contiguous"
-            nd = len(decodes)
-            bt_dec = meta.block_tables[decodes].contiguous()
-            cur_dec = torch.tensor([seq_lens[i] - 1 for i in decodes], dtype=torch.int32).to(self.device)
-            if nd not in self._dec_ws:
-                self._dec_ws[nd] = ops.decode_attention_workspace(nd, nkv, llm.decode_splits, self.device)
-        ws = llm._ws(max(T, 16))
-        xn, qkv, attn, xn2 = ws["xn"][:T], ws["qkv"][:T], ws["attn"][:T], ws["xn2"][:T]
-        ids, tw = ws["ids"][:T], ws["tw"][:T]
-        perm, rtok, rw = ws["perm"][:2 * T], ws["rtok"][:2 * T], ws["rw"][:2 * T]
-        xp, act, yp = ws["xp"][:2 * T], ws["act"][:2 * T], ws["yp"][:2 * T]
+        assert qsl[-1] == h.shape[0] and len(seq_lens) == len(qsl) - 1
+        attention = LayerAttention.of_batch(qsl, seq_lens, meta.block_tables, self.block_size, self._decode_workspace)
         slots = meta.slot_mapping.to(device=self.device, dtype=torch.int32)
-        layers = w["layers"]
-        ops.rmsnorm(h, layers[0]["ln1"], c.rms_norm_eps, out=xn)
-        for li, lw in enumerate(layers):
-            kc = kv_caches[li][0].reshape(-1, nkv, D)       # engine-owned pages, vLLM flash layout
-            vc = kv_caches[li][1].reshape(-1, nkv, D)
-            ops.linear_qkv_rope(xn, lw["wqkv"], qkv, positions, slots, w["rope"], kc, vc, nq, nkv, D)
-            for r0, n in prefills:
-                q = qkv[r0:r0 + n]
-                ops.attention(q, q[:, nq * D:], q[:, (nq + nkv) * D:], attn[r0:r0 + n], (0, W_, D), (0, W_, D),
-                              (0, W_, D), (0, nq * D, D), 1, nq, nkv, n, n, D, D, None, True, D ** -0.5)
-            if paged is not None:
-                ops.attention_prefill_paged(qkv, kc, vc, paged, attn, nq, nkv, D, D ** -0.5)
-            if decodes:
-                ops.decode_attention(qkv[d0:d0 + nd], kc, vc, bt_dec, cur_dec, attn[d0:d0 + nd], self._dec_ws[nd], nq,
-                                     nkv, D, self.block_size, llm.decode_splits, D ** -0.5, q_stride=W_)
-            ops.linear(attn, lw["wo"], residual=h, out=h)
-            ops.moe_router(h, lw["ln2"], lw["gate"], xn2, ids, tw, c.rms_norm_eps)
-            ops.moe_align(ids, tw, ws["offs"], perm, rtok, rw, T, E)
-            ops.row_copy(xn2, rtok, None, xp, 2 * T)
-            ops.moe_gate_up(xp, lw["w13"], act, ws["offs"], 2 * T)
-            ops.moe_down(act, lw["w2"], yp, ws["offs"], rw, 2 * T)
-            nxt = layers[li + 1]["ln1"] if li + 1 < len(layers) else w["norm"]
-            ops.moe_combine(h, yp, perm, nxt, xn, c.rms_norm_eps)
-        return xn.clone()                                   # final RMSNorm(h)
+        # engine-owned pages, vLLM flash layout
+        k = [kv[0].reshape(-1, c.num_key_value_heads, c.head_dim) for kv in kv_caches]
+        v = [kv[1].reshape(-1, c.num_key_value_heads, c.head_dim) for kv in kv_caches]
+        return self.llm.run_layers(h, positions, slots, k, v, attention, final_norm=True).clone()   # final RMSNorm(h)
+
+    def _decode_workspace(self, n: int) -> torch.Tensor:
+        if n not in self._dec_ws:
+            nkv = self.config.llm.num_key_value_heads
+            self._dec_ws[n] = ops.decode_attention_workspace(n, nkv, self.llm.decode_splits, self.device)
+        return self._dec_ws[n]
 
     # ------------------------------------------------------------------------------------------ logits / sampling
     @torch.no_grad()
