@@ -267,6 +267,19 @@ int vita_argmax_rows(const void* logits, uint64_t* best, int64_t B, int64_t V, v
 int vita_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
                      const int32_t* top_k, const float* top_p, const uint64_t* seed, const int32_t* counter,
                      uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows, void* stream);
+/* vita_sample_rows plus log-probabilities over the processed row (the logits for greedy rows; x = l / T over the kept
+ * set and -inf outside it otherwise; contract in vita_b200/sampling.py).  target (may be NULL): [B] i32; a row with
+ * target[b] in [0, V) draws nothing, leaves the greedy word in best[b] and scores target[b] (prompt rows: the next
+ * prompt token); other rows score the token they choose.  Per row: logprob f32 (log-sum-exp from u64 fixed-point
+ * masses: independent of summation order and batch position), rank i32 (1 + kept tokens with a strictly greater
+ * logit), and the n_top (0 .. 20, <= V) largest logits (lowest index first on ties) as top_ids i32 / top_logprobs f32
+ * [.., top_ld].  Output row of request b: b when out_rows == 0, else b * out_rows + counter[b] (skipped outside
+ * [0, out_rows)), so a device-resident log works under CUDA-graph replay. */
+int vita_sample_rows_logprobs(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
+                              const int32_t* top_k, const float* top_p, const uint64_t* seed, const int32_t* counter,
+                              const int32_t* target, uint64_t* best, void* scores, int64_t score_ld,
+                              int64_t score_rows, float* logprob, int32_t* rank, int32_t* top_ids,
+                              float* top_logprobs, int64_t n_top, int64_t top_ld, int64_t out_rows, void* stream);
 /* ---- greedy decode step on the tensor cores (wgmma swap-AB GEMV, stream-K) ---------------------------------
  * Every linear of the decode step as a weight-streaming GEMV on the tensor cores: the weight tile is the M operand of
  * wgmma and the activation vector as row 0 of a 16-wide N operand; (row-block, k-block) units are split evenly

@@ -37,6 +37,8 @@ SIGNATURES = {
     "vita_decode_slots": (c_int, [P, P, P, I64, I64, I64, P]),
     "vita_argmax_rows": (c_int, [P, P, I64, I64, P]),
     "vita_sample_rows": (c_int, [P, I64, I64, I64, P, P, P, P, P, P, P, I64, I64, P]),
+    "vita_sample_rows_logprobs": (c_int, [P, I64, I64, I64, P, P, P, P, P, P, P, P, I64, I64, P, P, P, P, I64, I64,
+                                          I64, P]),
     "vita_moe_router": (c_int, [P, P, P, P, P, P, I64, I64, I64, c_float, P]),
     "vita_moe_align": (c_int, [P, P, P, P, P, P, P, I64, I64, P]),
     "vita_moe_gemm_down_ep": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, P]),

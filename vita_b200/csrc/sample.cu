@@ -13,6 +13,14 @@
 // ordered keys of the logits (two 256-bin passes each): top-k over counts, top-p over fixed-point masses
 // exp(x_r - x_max) * 2^40 summed as u64 (integer sums: the result does not depend on the order of the additions).
 //
+// Log-probabilities (the LOGPROBS variant, vita_sample_rows_logprobs): over the processed row -- the logits for greedy
+// rows, x_r over the kept set and -inf outside it otherwise --
+//   logprob(r) = x_r - x_max - log(Z * 2^-40), Z = sum over the kept set of the fixed-point masses above (u64);
+//   rank(r) = 1 + #{kept tokens with a strictly greater logit}; top-N = the N largest logits, lowest index first on
+//   ties (the N-th largest comes from the same radix selection as top-k, with k = N).  Both compare the ordered keys
+//   with -0.0 read as +0.0, so equal logits are equal.
+// A row with a target id scores that token and draws nothing (prompt rows: the next prompt token).
+//
 // Reference call sites: vLLM's Sampler (web_demo/vllm_tools/vllm_file/mixtral.py:1180-1186) and the sampling loop of
 // HF generate() (video_audio_demo.py:257-270: TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper ->
 // multinomial).
@@ -82,8 +90,13 @@ __device__ __forceinline__ unsigned long long block_max_u64(unsigned long long v
     return red[0];
 }
 
+// -0.0 and +0.0 are one value to ranks and top-N: the key of -0.0 (0x7FFF) is read as that of +0.0
+__device__ __forceinline__ uint32_t canon_key(uint32_t k) { return k == 0x7FFFu ? 0x8000u : k; }
+
 // Histogram over the keys >= floor_key: high bytes (hi_bin < 0) or the low bytes of the keys whose high byte is
 // hi_bin.  Weight 1 (counts) or the fixed-point mass exp(x - x_max) * 2^40.  Result in tot[256].
+// CANON (counts only): over canon_key(key), with the lanes of a warp that hit one bin adding once.
+template <bool CANON = false>
 __device__ void sample_hist(const uint16_t* keys, int V, unsigned long long* whist, unsigned long long* tot,
                             int hi_bin, uint32_t floor_key, bool mass, float T, float x_max) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -91,7 +104,20 @@ __device__ void sample_hist(const uint16_t* keys, int V, unsigned long long* whi
 #pragma unroll
     for (int j = 0; j < 8; ++j) h[lane + 32 * j] = 0ull;
     __syncwarp();
-    for (int i = threadIdx.x; i < V; i += kSampleThreads) {
+    if constexpr (CANON) {
+        // every lane runs every iteration (the bound is uniform), so the whole warp takes part in the match
+        for (int base = 0; base < V; base += kSampleThreads) {
+            const int i = base + static_cast<int>(threadIdx.x);
+            int bin = -1;
+            if (i < V) {
+                const uint32_t k = canon_key(keys[i]);
+                if (hi_bin < 0 || static_cast<int>(k >> 8) == hi_bin) bin = static_cast<int>(hi_bin < 0 ? (k >> 8) : (k & 255u));
+            }
+            const unsigned peers = __match_any_sync(0xffffffffu, bin);
+            if (bin >= 0 && lane == __ffs(peers) - 1) atomicAdd(h + bin, static_cast<unsigned long long>(__popc(peers)));
+        }
+    }
+    for (int i = threadIdx.x; i < V && !CANON; i += kSampleThreads) {
         const uint32_t k = keys[i];
         if (k < floor_key) continue;
         if (hi_bin >= 0 && static_cast<int>(k >> 8) != hi_bin) continue;
@@ -148,12 +174,130 @@ __device__ void sample_search(const unsigned long long* tot, unsigned long long 
     if (lane == 0) { *res_bin = bin; *res_above = ab; *res_total = total; }
 }
 
+__device__ __forceinline__ unsigned long long block_sum_u64(unsigned long long v, unsigned long long* red) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    __syncthreads();                                    // red may still be read from a previous reduction
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        v = red[threadIdx.x];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (threadIdx.x == 0) red[0] = v;
+    }
+    __syncthreads();
+    return red[0];
+}
+
+// Outputs of the LOGPROBS variant.  Output row of request b: b when rows == 0, else b * rows + counter[b] (nothing is
+// written when the counter is outside [0, rows)), like the score log.
+struct LogprobArgs {
+    const int* target;          // [B] or null: a row with target[b] in [0, V) scores that token and draws nothing
+    float* logprob;             // [out rows]
+    int* rank;                  // [out rows]
+    int* top_ids;               // [out rows, top_ld] (n_top > 0)
+    float* top_logprobs;        // [out rows, top_ld] (n_top > 0)
+    int n_top, top_ld, rows;
+};
+constexpr int kMaxTopLogprobs = 20;
+
+// x of a staged key: l / T (SCALED) or l (greedy rows)
+template <bool SCALED>
+__device__ __forceinline__ float key_x(uint32_t k, float T) {
+    if constexpr (SCALED) return __fdiv_rn(key_value(k), T);
+    else return key_value(k);
+}
+
+// Logprob, rank and top-N of token `idx` over the processed row (kept set = keys >= thr).  Every thread calls it.
+template <bool SCALED>
+__device__ void write_logprobs(const uint16_t* keys, int V, uint32_t thr, float T, float x_max, int idx,
+                                            int n, int b, const LogprobArgs& lp, unsigned long long* whist,
+                                            unsigned long long* tot, unsigned long long* red, int* s_bin,
+                                            unsigned long long* s_above, unsigned long long* s_total) {
+    __shared__ int s_top[kMaxTopLogprobs];
+    __shared__ int s_cnt, s_wcnt[kSampleWarps];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t kt = canon_key(keys[idx]), kept_t = keys[idx];
+    // Z over the kept set (order-independent u64 sum) and the kept tokens strictly above the scored one
+    unsigned long long z = 0ull, gt = 0ull;
+    for (int i = tid; i < V; i += kSampleThreads) {
+        const uint32_t k = keys[i];
+        if (k < thr) continue;
+        z += __float2ull_rn(expf(key_x<SCALED>(k, T) - x_max) * 0x1p40f);
+        gt += canon_key(k) > kt ? 1ull : 0ull;
+    }
+    z = block_sum_u64(z, red);
+    gt = block_sum_u64(gt, red);
+    const float log_z = logf(__ull2float_rn(z) * 0x1p-40f);
+    auto logprob_of = [&](uint32_t k) { return k >= thr ? (key_x<SCALED>(k, T) - x_max) - log_z : -INFINITY; };
+
+    long long row = b;
+    if (lp.rows > 0) {
+        if (n < 0 || n >= lp.rows) return;               // uniform over the block
+        row = static_cast<long long>(b) * lp.rows + n;
+    }
+    if (tid == 0) {
+        lp.logprob[row] = logprob_of(kept_t);
+        lp.rank[row] = 1 + static_cast<int>(gt);
+    }
+    const int N = lp.n_top;
+    if (N <= 0) return;
+    // the N-th largest key (radix selection as for top-k), then every key above it and the lowest-index ties
+    sample_hist<true>(keys, V, whist, tot, -1, 0u, false, 1.0f, 0.0f);
+    sample_search(tot, 0ull, static_cast<double>(N), s_bin, s_above, s_total);
+    __syncthreads();
+    const int hb = *s_bin;
+    const unsigned long long ab = *s_above;
+    sample_hist<true>(keys, V, whist, tot, hb, 0u, false, 1.0f, 0.0f);
+    sample_search(tot, ab, static_cast<double>(N), s_bin, s_above, s_total);
+    if (tid == 0) s_cnt = 0;
+    __syncthreads();
+    const uint32_t thr_n = (static_cast<uint32_t>(hb) << 8) | static_cast<uint32_t>(*s_bin);
+    const int above = static_cast<int>(*s_above);        // keys > thr_n: fewer than N
+    for (int i = tid; i < V; i += kSampleThreads)
+        if (canon_key(keys[i]) > thr_n) s_top[atomicAdd(&s_cnt, 1)] = i;
+    int need = N - above;                                // ties at thr_n, taken in index order
+    for (int base = 0; base < V && need > 0; base += kSampleThreads) {
+        const int i = base + tid;
+        const bool tie = i < V && canon_key(keys[i]) == thr_n;
+        const unsigned bal = __ballot_sync(0xffffffffu, tie);
+        if (lane == 0) s_wcnt[warp] = __popc(bal);
+        __syncthreads();
+        int before = 0, total = 0;
+        for (int w = 0; w < kSampleWarps; ++w) {
+            const int c = s_wcnt[w];
+            before += w < warp ? c : 0;
+            total += c;
+        }
+        const int r = before + __popc(bal & ((1u << lane) - 1u));
+        if (tie && r < need) s_top[N - need + r] = i;
+        need -= total < need ? total : need;
+        __syncthreads();                                 // s_wcnt is rewritten by the next chunk
+    }
+    __syncthreads();
+    if (tid < N) {                                       // order: key descending, index ascending
+        const int i = s_top[tid];
+        const uint32_t k = canon_key(keys[i]);
+        int pos = 0;
+        for (int j = 0; j < N; ++j) {
+            const int o = s_top[j];
+            const uint32_t ko = canon_key(keys[o]);
+            pos += (ko > k || (ko == k && o < i)) ? 1 : 0;
+        }
+        const long long at = row * lp.top_ld + pos;
+        lp.top_ids[at] = i;
+        lp.top_logprobs[at] = logprob_of(keys[i]);
+    }
+}
+
+template <bool LOGPROBS>
 __global__ void __launch_bounds__(kSampleThreads, 1)
 sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, const float* __restrict__ temperature,
                    const int* __restrict__ top_k, const float* __restrict__ top_p,
                    const unsigned long long* __restrict__ seed, const int* __restrict__ counter,
                    unsigned long long* __restrict__ best, __nv_bfloat16* __restrict__ scores, long long score_ld,
-                   int score_rows, int vec) {
+                   int score_rows, int vec, LogprobArgs lp) {
     extern __shared__ __align__(16) uint8_t smem_s[];
     unsigned long long* whist = reinterpret_cast<unsigned long long*>(smem_s);
     uint16_t* keys = reinterpret_cast<uint16_t*>(smem_s + kSampleHistBytes);
@@ -173,6 +317,11 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
     const float p = top_p[b];
     const unsigned long long key = seed[b];
     const int n = counter[b];
+    int tgt = -1;
+    if constexpr (LOGPROBS) {
+        if (lp.target != nullptr) tgt = lp.target[b];
+        if (tgt >= V) tgt = -1;
+    }
 
     // stage the row as ordered keys; greedy arg-max on the way (largest key, first index)
     const __nv_bfloat16* row = logits + static_cast<long long>(b) * ld;
@@ -211,10 +360,18 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
         if (tid == 0) best[b] = arg;
         if (srow != nullptr)
             for (int i = tid; i < V; i += kSampleThreads) srow[i] = __float2bfloat16(key_value(keys[i]));
-        return;
+        if constexpr (!LOGPROBS) return;
     }
     const uint32_t ord = static_cast<uint32_t>(arg >> 32);     // undo pack_score's float ordering, then re-key
     const uint32_t max_key = bf16_key(((ord & 0x80000000u) ? (ord & 0x7FFFFFFFu) : ~ord) >> 16);
+    if constexpr (LOGPROBS) {
+        if (greedy) {                                    // the processed row is the logits: x = l, every token kept
+            const int idx = tgt >= 0 ? tgt : static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(arg & 0xFFFFFFFFull));
+            write_logprobs<false>(keys, V, 0u, 1.0f, key_value(max_key), idx, n, b, lp, whist, tot, red, &s_bin,
+                                  &s_above, &s_total);
+            return;
+        }
+    }
     const float x_max = __fdiv_rn(key_value(max_key), T);
 
     // top-k threshold: the k-th largest key
@@ -272,6 +429,7 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
             kept[e] = i < V && kk >= thr;
             x[e] = __fdiv_rn(key_value(kk), T);
             need |= kept[e] && x[e] >= x_floor;
+            if constexpr (LOGPROBS) need &= tgt < 0;    // a scored row draws nothing
             if (srow != nullptr && i < V) srow[i] = kept[e] ? __float2bfloat16(x[e]) : __float2bfloat16(-INFINITY);
         }
         if (!need) continue;
@@ -285,20 +443,35 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
         }
     }
     const unsigned long long win = block_max_u64(loc, red);
+    if constexpr (LOGPROBS) {
+        if (tgt >= 0) {                                  // a scored row leaves the greedy word in best
+            if (tid == 0) best[b] = arg;
+            write_logprobs<true>(keys, V, thr, T, x_max, tgt, n, b, lp, whist, tot, red, &s_bin, &s_above, &s_total);
+            return;
+        }
+    }
     // the winner's packed word keeps the arg-max layout: (bf16 logit as float, ~index)
     if (tid == 0) {
         const int idx = static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(win & 0xFFFFFFFFull));
         best[b] = pack_score(key_value(keys[idx]), idx);
     }
+    if constexpr (LOGPROBS)
+        write_logprobs<true>(keys, V, thr, T, x_max,
+                             static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(win & 0xFFFFFFFFull)), n, b, lp,
+                             whist, tot, red, &s_bin, &s_above, &s_total);
 }
 
 }  // namespace vita
 
 using namespace vita;
 
-extern "C" int vita_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
-                                const int32_t* top_k, const float* top_p, const uint64_t* seed, const int32_t* counter,
-                                uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows, void* stream) {
+namespace {
+
+template <bool LOGPROBS>
+int launch_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
+                       const int32_t* top_k, const float* top_p, const uint64_t* seed, const int32_t* counter,
+                       uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows, const LogprobArgs& lp,
+                       void* stream) {
     VITA_REQUIRE(V > 0 && ld >= V, "need 0 < V <= ld");
     VITA_REQUIRE(temperature && top_k && top_p && seed && counter && best, "parameter arrays are required");
     VITA_REQUIRE(scores == nullptr || (score_ld >= V && score_rows > 0), "score log: need score_ld >= V, rows > 0");
@@ -311,7 +484,7 @@ extern "C" int vita_sample_rows(const void* logits, int64_t ld, int64_t B, int64
         cudaFuncAttributes fa{};
         int rc = check_cuda(cudaGetDevice(&dev), "sample_rows");
         if (!rc) rc = check_cuda(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev), "sample_rows");
-        if (!rc) rc = check_cuda(cudaFuncGetAttributes(&fa, sample_rows_kernel), "sample_rows");
+        if (!rc) rc = check_cuda(cudaFuncGetAttributes(&fa, sample_rows_kernel<LOGPROBS>), "sample_rows");
         if (rc) return rc;
         dyn_limit = static_cast<size_t>(optin) > fa.sharedSizeBytes ? static_cast<size_t>(optin) - fa.sharedSizeBytes : 0;
     }
@@ -321,7 +494,8 @@ extern "C" int vita_sample_rows(const void* logits, int64_t ld, int64_t B, int64
                                         " on this device)");
     static size_t configured = 0;
     if (smem > configured) {
-        const int rc = check_cuda(cudaFuncSetAttribute(sample_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        const int rc = check_cuda(cudaFuncSetAttribute(sample_rows_kernel<LOGPROBS>,
+                                                       cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                        static_cast<int>(smem)), "sample_rows");
         if (rc) return rc;
         configured = smem;
@@ -329,11 +503,35 @@ extern "C" int vita_sample_rows(const void* logits, int64_t ld, int64_t B, int64
     const int vec = (V % 8 == 0 && ld % 8 == 0 && aligned16(logits)) ? 1 : 0;
     // launched as a programmatic dependent of the LM head: the kernel waits (griddepcontrol.wait) before reading the
     // logits and never triggers its own dependents early, so the next step starts after its last write of `best`
-    cudaError_t e = launch_chain(sample_rows_kernel, dim3(static_cast<unsigned>(B)), dim3(kSampleThreads), smem,
+    cudaError_t e = launch_chain(sample_rows_kernel<LOGPROBS>, dim3(static_cast<unsigned>(B)), dim3(kSampleThreads), smem,
                                  static_cast<cudaStream_t>(stream), BF16C(logits), (long long)ld, (int)V, temperature,
                                  top_k, top_p, reinterpret_cast<const unsigned long long*>(seed), counter,
                                  reinterpret_cast<unsigned long long*>(best), static_cast<__nv_bfloat16*>(scores),
-                                 (long long)score_ld, (int)score_rows, vec);
+                                 (long long)score_ld, (int)score_rows, vec, lp);
     if (e != cudaSuccess) return check_cuda(e, "sample_rows");
     return check_launch("sample_rows");
+}
+
+}  // namespace
+
+extern "C" int vita_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
+                                const int32_t* top_k, const float* top_p, const uint64_t* seed, const int32_t* counter,
+                                uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows, void* stream) {
+    return launch_sample_rows<false>(logits, ld, B, V, temperature, top_k, top_p, seed, counter, best, scores, score_ld,
+                                     score_rows, LogprobArgs{}, stream);
+}
+
+extern "C" int vita_sample_rows_logprobs(const void* logits, int64_t ld, int64_t B, int64_t V,
+                                         const float* temperature, const int32_t* top_k, const float* top_p,
+                                         const uint64_t* seed, const int32_t* counter, const int32_t* target,
+                                         uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows,
+                                         float* logprob, int32_t* rank, int32_t* top_ids, float* top_logprobs,
+                                         int64_t n_top, int64_t top_ld, int64_t out_rows, void* stream) {
+    VITA_REQUIRE(logprob && rank, "logprob and rank outputs are required");
+    VITA_REQUIRE(n_top >= 0 && n_top <= kMaxTopLogprobs && n_top <= V, "need 0 <= n_top <= min(20, V)");
+    VITA_REQUIRE(n_top == 0 || (top_ids && top_logprobs && top_ld >= n_top), "top-N outputs: need top_ld >= n_top");
+    VITA_REQUIRE(out_rows >= 0, "out_rows must be >= 0");
+    const LogprobArgs lp{target, logprob, rank, top_ids, top_logprobs, (int)n_top, (int)top_ld, (int)out_rows};
+    return launch_sample_rows<true>(logits, ld, B, V, temperature, top_k, top_p, seed, counter, best, scores, score_ld,
+                                    score_rows, lp, stream);
 }

@@ -30,9 +30,9 @@ time is admitted this way; it sits in slot n_active, right behind the prefix, an
 request retires.  Its duplex events are decided after the final chunk, when its first token is known.  With nothing
 running the whole prompt goes in at once.
 
-`ContinuousBatcher` only talks to an `engine` object (prefill / step / swap / read_tokens / reset_slot / first_token, and
-begin_prefill / prefill_rows for chunked admission), so the policy is unit-tested on the CPU with a deterministic
-stand-in; `DecoderEngine` binds it to `VITAMixtralForCausalLM`.
+`ContinuousBatcher` only talks to an `engine` object (prefill / step / swap / read_tokens / reset_slot / first_token,
+begin_prefill / prefill_rows for chunked admission, and read_logprobs only for requests that ask for logprobs), so the
+policy is unit-tested on the CPU with a deterministic stand-in; `DecoderEngine` binds it to `VITAMixtralForCausalLM`.
 """
 from __future__ import annotations
 
@@ -41,7 +41,7 @@ from typing import Callable, Dict, List, Optional, Sequence
 
 import torch
 
-from .sampling import SamplingParams
+from .sampling import SamplingParams, TokenLogprobs
 
 
 @dataclass
@@ -54,12 +54,14 @@ class Request:
     session: Optional[int] = None       # duplex: queries of one conversation; a real query interrupts the running answer
     negative_token_id: Optional[int] = None   # duplex: state token `<2>`; a query answering with it is dropped at once
     sampling: Optional[SamplingParams] = None  # None = greedy (vita_b200/sampling.py: from_hf / from_vllm build one)
+    logprobs: Optional[int] = None      # top-N (0 .. 20) of each kept token's logprob record; None = no logprobs
     # filled in by the batcher
     outcome: str = ""                   # "finished" | "negative" | "interrupted"
     steps: int = 0
     admitted_step: int = -1
     finished_step: int = -1
     tokens: List[int] = field(default_factory=list)
+    token_logprobs: List[TokenLogprobs] = field(default_factory=list)   # one per kept token (with `logprobs`)
 
 
 def swap_rows(tensors: Sequence[torch.Tensor], i: int, j: int) -> None:
@@ -133,6 +135,7 @@ class ContinuousBatcher:
             if r.negative_token_id is not None and first == r.negative_token_id:
                 # negative audio: never enters the decode batch (the slot is simply reused by the next arrival)
                 r.tokens, r.finished_step, r.outcome = [first], step, "negative"
+                self._logprobs(r, slot)
                 done[r.rid] = r.tokens
                 return
             if r.session is not None:                        # a real query: interrupt the running answer
@@ -140,6 +143,7 @@ class ContinuousBatcher:
                     old = active[old_slot]
                     old.tokens = self.engine.read_tokens(old_slot)[: min(old.steps, old.max_new_tokens)]
                     old.finished_step, old.outcome = step, "interrupted"
+                    self._logprobs(old, old_slot)
                     done[old.rid] = old.tokens
                     last = len(active) - 1
                     # the new request sits in slot len(active) (not yet appended): move it down with the rest
@@ -149,6 +153,11 @@ class ContinuousBatcher:
                     active.pop()
                     self.engine.swap(last, last + 1)          # keep the new request right behind the prefix
         active.append(r)
+
+    def _logprobs(self, r: Request, slot: int) -> None:
+        """The logprob records of r's kept tokens, read before its slot is reused (only for requests that ask)."""
+        if r.logprobs is not None:
+            r.token_logprobs = self.engine.read_logprobs(slot, r.tokens, r.logprobs)
 
     def _retire(self, active: List[Request], done: Dict[int, List[int]], step: int, admitting: bool = False) -> None:
         finished = []
@@ -161,6 +170,7 @@ class ContinuousBatcher:
                 cut = r.max_new_tokens
             if cut is not None:
                 r.tokens, r.finished_step, r.outcome = toks[: min(cut, r.max_new_tokens)], step, "finished"
+                self._logprobs(r, slot)
                 finished.append(slot)
         for slot in sorted(finished, reverse=True):     # highest slot first: the swap partner is never a finished one
             last = len(active) - 1
@@ -183,7 +193,7 @@ class DecoderEngine:
         the batched GEMM step (faster; the two paths round differently, so tokens are no longer batch-invariant)."""
         self.model, self.llm, self.use_graph, self.overrun = model, model.llm, use_graph, overrun
         self.lone_fast_path = lone_fast_path
-        self._adm = None                    # (prompt rows, sampled) of the request being admitted in chunks
+        self._adm = None                    # (prompt rows, sampled, logprobs) of the request admitted in chunks
         c = self.llm.cache
         self._slot_tensors = [c.block_table, c.slot_map, c.cache_len, c.cur_pos, self.llm.best, self.llm.token_log,
                               self.llm.gen_count, *self.llm.sampling.tensors]
@@ -198,8 +208,9 @@ class DecoderEngine:
         p = request.payload
         emb, lens = self.model._embeds_for(p["input_ids"], p.get("images"), p.get("audios"))
         self._check(request, int(lens[0]))
-        self.llm.sampling.set(slot, request.sampling)
-        self.llm.prefill(emb[0, : lens[0]].contiguous(), slot=slot, sampled=request.sampling is not None)
+        self.llm.sampling.set(slot, request.sampling, request.logprobs)
+        self.llm.prefill(emb[0, : lens[0]].contiguous(), slot=slot, sampled=request.sampling is not None,
+                         logprobs=self.llm.sampling.log_width(slot, 1))
 
     def begin_prefill(self, slot: int, request: Request) -> int:
         """Chunked admission: run the encoders and the splice once, keep the prompt rows; returns their count."""
@@ -207,14 +218,14 @@ class DecoderEngine:
         emb, lens = self.model._embeds_for(p["input_ids"], p.get("images"), p.get("audios"))
         S = int(lens[0])
         self._check(request, S)
-        self.llm.sampling.set(slot, request.sampling)
-        self._adm = (emb[0, :S].contiguous(), request.sampling is not None)
+        self.llm.sampling.set(slot, request.sampling, request.logprobs)
+        self._adm = (emb[0, :S].contiguous(), request.sampling is not None, self.llm.sampling.log_width(slot, 1))
         return S
 
     def prefill_rows(self, slot: int, start: int, n: int, final: bool) -> None:
         """Prompt rows [start, start + n) of the request being admitted into `slot` (which holds its first `start`)."""
-        rows, sampled = self._adm
-        self.llm.prefill(rows[start:start + n], slot=slot, sampled=sampled, start=start, final=final)
+        rows, sampled, logprobs = self._adm
+        self.llm.prefill(rows[start:start + n], slot=slot, sampled=sampled, start=start, final=final, logprobs=logprobs)
         if final:
             self._adm = None
 
@@ -227,18 +238,27 @@ class DecoderEngine:
     def step(self, n_active: int) -> None:
         # the sampled step when any active request samples (its greedy rows keep the greedy tokens), else the greedy one
         sampled = self.llm.sampling.any_sampled(n_active)
+        # the sampler path also when a running request asks for logprobs (greedy rows keep their tokens)
+        logprobs = self.llm.sampling.log_width(0, n_active)
         if n_active == 1 and self.lone_fast_path:      # a lone request takes the weight-streaming GEMV chain (2 experts read, not a GEMM tile)
-            self.llm.decode_step(1, use_graph=self.use_graph, sampled=sampled)
+            self.llm.decode_step(1, use_graph=self.use_graph, sampled=sampled, logprobs=logprobs)
         else:
-            self.llm.decode_step_batched(n_active, use_graph=self.use_graph, sampled=sampled)
+            self.llm.decode_step_batched(n_active, use_graph=self.use_graph, sampled=sampled, logprobs=logprobs)
 
     def swap(self, i: int, j: int) -> None:
         swap_rows(self._slot_tensors, i, j)
         if i != j:
             self.llm.sampling.swap(i, j)
+            if self.llm.lp_log is not None:          # the logprob log rows move with their request
+                swap_rows(self.llm.lp_log, i, j)
 
     def read_tokens(self, slot: int) -> List[int]:
         return self.llm.generated_tokens(slot)
+
+    def read_logprobs(self, slot: int, tokens: List[int], n_top: int) -> List[TokenLogprobs]:
+        """The logprob records of `tokens`, the kept tokens of the request in `slot` (its first one included, which
+        the token log does not hold yet when a negative query is dropped right after its prefill)."""
+        return self.llm.read_logprobs(slot, tokens, n_top)
 
     def first_token(self, slot: int) -> int:
         """arg-max of the prompt's last position (packed as (logit, ~index) by the LM-head kernel); one host sync"""

@@ -6,6 +6,7 @@ web_demo/vllm_tools/vllm_file/mixtral.py:375-628).  Host code only sequences ker
 """
 from __future__ import annotations
 
+import gc
 import os
 from dataclasses import dataclass
 from typing import Callable, List, Optional, Sequence, Tuple
@@ -14,7 +15,7 @@ import torch
 
 from .. import ops
 from ..config import LLMConfig
-from ..sampling import SlotSampling
+from ..sampling import MAX_LOGPROBS, SlotSampling, logprob_records
 
 BF16 = torch.bfloat16
 
@@ -160,6 +161,7 @@ class MixtralDecoder:
         self.chain_mem = torch.zeros(2 + 5 * cfg.num_hidden_layers, dtype=torch.int64, device=dev)
         self._graphs = {}             # single-sequence decode step: captured CUDA graph per (B, want_logits[, sampled])
         self.scores_buf = None        # [max_new_tokens + 1, V] logits log of slot 0 (generate(output_scores=True))
+        self.lp_log = None            # per-slot logprob log (enable_logprob_log)
         self._bgraphs = {}            # batched decode step: captured CUDA graph per (batch size, sampled)
         self.d_slots = torch.zeros(B, dtype=torch.int32, device=dev)
         self._prefill_ws = {}
@@ -290,14 +292,15 @@ class MixtralDecoder:
     @torch.no_grad()
     def prefill(self, inputs_embeds: torch.Tensor, slot: int = 0, all_logits: bool = False,
                 want_last_logits: bool = False, sampled: bool = False, scores: Optional[torch.Tensor] = None,
-                start: int = 0, final: bool = True):
+                start: int = 0, final: bool = True, logprobs: Optional[int] = None):
         """One sequence: inputs_embeds [S, H] bf16 (consumed as the residual stream, modified in place).
 
         Appends S tokens to the KV cache of batch slot `slot` (which must be empty), leaves the arg-max of the last
         position in self.best[slot] (the first generated token) and returns logits [S, V] if `all_logits`.
         `sampled`: the first token is drawn instead (self.sampling's parameters of the slot, counter 0 =
         gen_count[slot] of the empty slot) from the last-row logits; `scores` [rows, V] receives the warped row at
-        row 0.
+        row 0.  `logprobs` (a log width, see `_sample`; None: none): the first token goes through the sampler (greedy
+        slots get the LM head's arg-max word) and its logprobs land in row 0 of the slot's logprob log.
 
         Chunked prefill / prefix reuse: `start` is the number of tokens the slot already holds (rows get positions
         start + i and attend the cached ones through the paged-KV attention kernel).  With `final` False the rows are
@@ -311,6 +314,8 @@ class MixtralDecoder:
                              f"per sequence")
         if sampled and self.ep_world > 1:
             raise ValueError("sampled decoding is single-GPU: the expert-parallel prefill serves greedy requests")
+        if logprobs is not None and self.ep_world > 1:
+            raise ValueError("logprobs are single-GPU: the expert-parallel prefill serves greedy requests")
         if (start > 0 or not final) and self.ep_world > 1:
             raise ValueError("chunked prefill is single-GPU: the expert-parallel prefill takes whole prompts")
         if self.ep_mode == "seq":
@@ -329,11 +334,12 @@ class MixtralDecoder:
             return ops.linear(xn, w["lm_head"]) if all_logits else None
         # first generated token: final norm + lm_head + arg-max on the last row only
         self.best[slot:slot + 1].zero_()
-        last_logits = self.d_logits[slot:slot + 1] if (want_last_logits or all_logits or sampled) else None
+        last_logits = self.d_logits[slot:slot + 1] if (want_last_logits or all_logits or sampled
+                                                             or logprobs is not None) else None
         ops.tc_lm_head_argmax(h[S - 1:], H, w["norm"], w["lm_head"], last_logits, self.best[slot:slot + 1], 1,
                               self.tc_ws, c.rms_norm_eps)
-        if sampled:
-            self._sample(slot, 1, scores)
+        if sampled or logprobs is not None:
+            self._sample(slot, 1, scores, logprobs)
         if all_logits:
             return ops.linear(xn, w["lm_head"])      # [S, V]; xn = final RMSNorm(h) written by the last combine
         return last_logits
@@ -416,12 +422,14 @@ class MixtralDecoder:
         return last_logits
 
     # ------------------------------------------------------------------------------------------ decode
-    def _decode_step_kernels(self, B: int, want_logits: bool, sampled: bool = False):
+    def _decode_step_kernels(self, B: int, want_logits: bool, sampled: bool = False,
+                             logprobs: Optional[int] = None):
         """One greedy token for slots [0, B): embed + per layer (qkv+RoPE+KV append -> paged attention -> o-proj ->
         router+gate/up -> down) + LM head with arg-max, 2 + 5 L launches chained by programmatic dependent launch.
         For B = 1 the kernels are additionally linked by completion counters (include/vita_b200.h, vita_chain_begin).
         `sampled`: the LM head writes the logits and the sampler draws the token from them (one launch more, after the
-        counter chain; with a score log it writes the warped row in place of the logits copy)."""
+        counter chain; with a score log it writes the warped row in place of the logits copy).  `logprobs`: the
+        sampler path as well, writing the logprob log too (greedy rows keep the LM head's arg-max word)."""
         c, w, cache = self.cfg, self.w, self.cache
         nq, nkv, D = c.num_attention_heads, c.num_key_value_heads, c.head_dim
         h = self.d_h[:B]
@@ -447,21 +455,49 @@ class MixtralDecoder:
                 if tracing:
                     self.route_trace.append((self.d_ids[:B].clone(), self.d_w[:B].clone()))
                 ops.decode_tc_moe_down(self.d_act[:B], lw["w2"], self.d_ids[:B], self.d_w[:B], h, ws, route, li + 1)
-            lg = self.d_logits[:B] if (want_logits or sampled) else None
+            lg = self.d_logits[:B] if (want_logits or sampled or logprobs is not None) else None
             ops.tc_lm_head_argmax(h, c.hidden_size, w["norm"], w["lm_head"], lg, self.best[:B], B, ws, c.rms_norm_eps)
         finally:
             if chained:
                 ops.chain_end()
-        if sampled:
-            self._sample(0, B, self.scores_buf if (want_logits and B == 1) else None)
+        if sampled or logprobs is not None:
+            self._sample(0, B, self.scores_buf if (want_logits and B == 1) else None, logprobs)
         else:
             self._log_scores(B, want_logits)
 
-    def _sample(self, s0: int, n: int, scores: Optional[torch.Tensor]):
-        """Draw the next token of slots [s0, s0 + n) from d_logits into best (counter = gen_count of the slot)."""
+    def _sample(self, s0: int, n: int, scores: Optional[torch.Tensor], logprobs: Optional[int] = None):
+        """Draw the next token of slots [s0, s0 + n) from d_logits into best (counter = gen_count of the slot).
+        `logprobs` (the log width, SlotSampling.log_width: 0 or 20): also write the token's logprob, rank and that
+        many top entries at row gen_count of each slot's logprob log."""
         sp, rows = self.sampling, slice(s0, s0 + n)
-        ops.sample_rows(self.d_logits[rows], sp.temperature[rows], sp.top_k[rows], sp.top_p[rows], sp.seed[rows],
-                        self.gen_count[rows], self.best[rows], scores)
+        if logprobs is None:
+            ops.sample_rows(self.d_logits[rows], sp.temperature[rows], sp.top_k[rows], sp.top_p[rows], sp.seed[rows],
+                            self.gen_count[rows], self.best[rows], scores)
+            return
+        lg = self.enable_logprob_log()
+        ops.sample_logprobs(self.d_logits[rows], sp.temperature[rows], sp.top_k[rows], sp.top_p[rows], sp.seed[rows],
+                            self.gen_count[rows], self.best[rows], lg[0][rows], lg[1][rows], lg[2][rows], lg[3][rows],
+                            logprobs, scores=scores)
+
+    def enable_logprob_log(self):
+        """Allocate the per-slot logprob log: (logprob f32 [B, R], rank i32 [B, R], top ids i32 [B, R, 20], top
+        logprobs f32 [B, R, 20]), R = the token log's length.  Row i of a slot belongs to its generated token i (row
+        index = gen_count, written on the device, so it works under CUDA-graph replay).  A step records the top 20 when
+        any of its requests asks for top entries (readers keep the N a request asked for), none otherwise."""
+        if self.lp_log is None:
+            B, R, dev = self.max_batch, self.token_log.shape[1], self.device
+            with torch.inference_mode(False):
+                self.lp_log = (torch.zeros(B, R, dtype=torch.float32, device=dev),
+                               torch.zeros(B, R, dtype=torch.int32, device=dev),
+                               torch.zeros(B, R, MAX_LOGPROBS, dtype=torch.int32, device=dev),
+                               torch.zeros(B, R, MAX_LOGPROBS, dtype=torch.float32, device=dev))
+        return self.lp_log
+
+    def read_logprobs(self, slot: int, tokens: Sequence[int], n_top: int):
+        """TokenLogprobs of the generated tokens of `slot` (`tokens`: the first len(tokens) of them, as the caller
+        holds them; the token log only receives a token when the next step consumes it), top-n_top each."""
+        lp, rk, ti, tl = (t[slot, :len(tokens)].cpu() for t in self.lp_log)
+        return logprob_records(tokens, lp, rk, ti, tl, n_top)
 
     def enable_score_log(self):
         """Allocate the per-step logits log (HF `output_scores=True`): row i holds the logits token i was chosen from.
@@ -491,20 +527,23 @@ class MixtralDecoder:
         return self.launches_per_decode_step + 1
 
     @torch.no_grad()
-    def decode_step(self, B: int = 1, use_graph: bool = True, want_logits: bool = False, sampled: bool = False):
+    def decode_step(self, B: int = 1, use_graph: bool = True, want_logits: bool = False, sampled: bool = False,
+                    logprobs: Optional[int] = None):
         """Generate one token for batch slots [0, B): consumes self.best, appends to token_log, leaves the next
         arg-max (or, `sampled`, the drawn token) in self.best.  With use_graph the whole step (2 + 5 * layers kernels,
         one more when sampled) replays as one CUDA graph."""
         assert self.ep_world == 1, "expert-parallel mode covers the prefill (BASELINE configs[3]); decode is replicated"
-        step = lambda: self._decode_step_kernels(B, want_logits, sampled)
+        step = lambda: self._decode_step_kernels(B, want_logits, sampled, logprobs)
         if not use_graph:
             step()
             return
         key = (B, want_logits, True) if sampled else (B, want_logits)    # greedy keys keep their (B, want_logits) form
+        if logprobs is not None:
+            key = (B, want_logits, sampled, "logprobs", logprobs)
         self._replay(self._graphs, key, step)
 
     # ------------------------------------------------------------------------------------------ batched decode
-    def _batched_step_kernels(self, B: int, sampled: bool = False):
+    def _batched_step_kernels(self, B: int, sampled: bool = False, logprobs: Optional[int] = None):
         """One token for each of B sequences through the GEMM path (weights of every touched expert are streamed once
         for the whole batch; BASELINE configs[4]).  The prefill's layer loop with M = B rows at B different
         positions and the paged decode attention."""
@@ -518,8 +557,8 @@ class MixtralDecoder:
                                    page_size=cache.page_size)
         xn = self.run_layers(h, cache.cur_pos[:B], slots, cache.k, cache.v, attention, final_norm=True)
         logits = ops.linear(xn, w["lm_head"], out=self.d_logits[:B])
-        if sampled:          # greedy rows (temperature 0) get argmax_rows' word: a mixed batch keeps their tokens
-            self._sample(0, B, None)
+        if sampled or logprobs is not None:   # greedy rows (temperature 0) get argmax_rows' word: a mixed batch keeps their tokens
+            self._sample(0, B, None, logprobs)
         else:
             ops.argmax_rows(logits, self.best[:B])
 
@@ -528,13 +567,15 @@ class MixtralDecoder:
         return 6 + 8 * self.cfg.num_hidden_layers
 
     @torch.no_grad()
-    def decode_step_batched(self, B: int, use_graph: bool = True, sampled: bool = False):
+    def decode_step_batched(self, B: int, use_graph: bool = True, sampled: bool = False,
+                            logprobs: Optional[int] = None):
         assert self.ep_world == 1 and 1 <= B <= self.max_batch
-        step = lambda: self._batched_step_kernels(B, sampled)
+        step = lambda: self._batched_step_kernels(B, sampled, logprobs)
         if not use_graph:
             step()
             return
-        self._replay(self._bgraphs, (B, sampled), step)   # one graph per batch size (continuous batching changes B)
+        key = (B, sampled, "logprobs", logprobs) if logprobs is not None else (B, sampled)
+        self._replay(self._bgraphs, key, step)   # one graph per batch size (continuous batching changes B)
 
     def _replay(self, graphs: dict, key, step):
         """Replay graphs[key], capturing `step` (a decode step that takes no host input) into it first: an eager
@@ -547,9 +588,17 @@ class MixtralDecoder:
             g = torch.cuda.CUDAGraph()
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                with torch.cuda.graph(g, stream=side):
-                    step()
+            # no garbage collection inside the capture: collecting an unreachable model destroys its CUDA graphs, and
+            # destroying a graph while a stream captures invalidates the capture
+            gc_enabled = gc.isenabled()
+            gc.disable()
+            try:
+                with torch.cuda.stream(side):
+                    with torch.cuda.graph(g, stream=side):
+                        step()
+            finally:
+                if gc_enabled:
+                    gc.enable()
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
             self._restore_state(snap)   # capture does not execute, but keep the invariant explicit

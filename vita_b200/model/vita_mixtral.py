@@ -15,7 +15,7 @@ import torch
 from .. import ops
 from ..config import VitaConfig, IMAGE_TOKEN_INDEX, AUDIO_TOKEN_INDEX
 from .internvit import InternViTVisionTower, VisionProjector
-from ..sampling import from_hf
+from ..sampling import check_logprobs, from_hf
 from .mixtral import MixtralDecoder
 from .whale import AudioEncoder
 
@@ -105,6 +105,7 @@ class CausalLMOutput:
 class GenerateOutput:
     sequences: torch.Tensor
     scores: Optional[tuple] = None
+    logprobs: Optional[tuple] = None      # generate(logprobs=N): one sampling.TokenLogprobs per generated token
 
 
 class CapturedEncoders:
@@ -334,27 +335,37 @@ class VITAMixtralForCausalLM:
 
         `requests`: list of dicts {"input_ids": [1, L], "images": ..., "audios": ...}, optionally with
         "sampling": {"temperature", "top_k", "top_p", "seed"} (as for generate(do_sample=True)); the others are greedy.
-        Each request is prefilled into its own paged-KV slot, then all of them advance one token per step through the
+        A request with "logprobs": N (0 .. 20) receives "token_logprobs": one sampling.TokenLogprobs per returned token
+        (as generate(logprobs=N)).  Each request is prefilled into its own paged-KV slot, then all of them advance one token per step through the
         batched decode step.  Returns the list of generated token lists.  `step_callback(step_index)` is called after
         every step launch (latency harnesses record CUDA events there)."""
         B = len(requests)
         if not 1 <= B <= self.llm.max_batch:
             raise ValueError(f"{B} requests do not fit max_batch = {self.llm.max_batch}")
         params = [None if r.get("sampling") is None else from_hf(True, **r["sampling"]) for r in requests]
+        n_top = [check_logprobs(r.get("logprobs")) for r in requests]
         if any(params) and self.llm.ep_world > 1:
             raise ValueError("sampled decoding is single-GPU (the expert-parallel mode serves greedy requests)")
+        if any(n is not None for n in n_top) and self.llm.ep_world > 1:
+            raise ValueError("logprobs are single-GPU (the expert-parallel mode serves greedy requests)")
         self.llm.reset()
         for b, r in enumerate(requests):
             emb, lens = self._embeds_for(r["input_ids"], r.get("images"), r.get("audios"))
             self.llm.check_capacity(lens[0], max_new_tokens)
-            self.llm.sampling.set(b, params[b])
-            self.llm.prefill(emb[0, : lens[0]].contiguous(), slot=b, sampled=params[b] is not None)
+            self.llm.sampling.set(b, params[b], n_top[b])
+            self.llm.prefill(emb[0, : lens[0]].contiguous(), slot=b, sampled=params[b] is not None,
+                             logprobs=self.llm.sampling.log_width(b, 1))
         sampled = any(p is not None for p in params)
+        logprobs = self.llm.sampling.log_width(0, B)
         for step in range(max_new_tokens):
-            self.llm.decode_step_batched(B, use_graph=use_graph, sampled=sampled)
+            self.llm.decode_step_batched(B, use_graph=use_graph, sampled=sampled, logprobs=logprobs)
             if step_callback is not None:
                 step_callback(step)
-        return [self.llm.generated_tokens(b)[:max_new_tokens] for b in range(B)]
+        out = [self.llm.generated_tokens(b)[:max_new_tokens] for b in range(B)]
+        for b, r in enumerate(requests):
+            if n_top[b] is not None:
+                r["token_logprobs"] = self.llm.read_logprobs(b, out[b], n_top[b])
+        return out
 
     def prepare_inputs_for_generation_original(self, input_ids, past_key_values=None, attention_mask=None,
                                                inputs_embeds=None, output_router_logits=False, **kwargs):
@@ -402,7 +413,7 @@ class VITAMixtralForCausalLM:
     def generate(self, input_ids, images=None, audios=None, do_sample=False, temperature=None, top_p=None,
                  num_beams=1, output_scores=False, return_dict_in_generate=True, max_new_tokens=16, use_cache=True,
                  stopping_criteria=None, eos_token_id: Optional[int] = None, use_graph: bool = True, sync_every: int = 16,
-                 top_k=None, seed: Optional[int] = None, **kw):
+                 top_k=None, seed: Optional[int] = None, logprobs: Optional[int] = None, **kw):
         """Greedy or sampled decode with the call signature of video_audio_demo.py:257-270.  `sequences` (on
         `input_ids.device`) echoes the prompt ids, placeholders included, followed by the new tokens
         (video_audio_demo.py:272-276).
@@ -411,6 +422,9 @@ class VITAMixtralForCausalLM:
         4.41's defaults 1.0, 50, 1.0; the policy is vita_b200/sampling.py).  `seed` (an extension) is the 64-bit stream
         key; without it one key is drawn from torch's default CPU generator, so `torch.manual_seed` makes a call
         reproducible.  With `output_scores` the scores are the warped rows, as HF returns them when sampling.
+        `logprobs=N` (an extension, 0 .. 20) fills `logprobs` with one sampling.TokenLogprobs per generated token: its
+        logprob and rank over the row it was chosen from and the N most likely tokens, computed on the GPU next to the
+        choice (greedy tokens are unchanged).
 
         The decode step replays as one CUDA graph whether or not `output_scores` is set: with scores the step appends
         its logits row to a device-resident log, and `scores` are views of that log (valid until the next call).
@@ -419,18 +433,25 @@ class VITAMixtralForCausalLM:
             raise ValueError("beam search is not supported (num_beams=1)")
         params = from_hf(do_sample, temperature, top_k, top_p, seed, **kw)
         sampled = params is not None
+        n_top = check_logprobs(logprobs)
+        want_lp = n_top is not None
         if sampled and self.llm.ep_world > 1:
             raise ValueError("sampled decoding is single-GPU (the expert-parallel mode serves greedy requests)")
+        if want_lp and self.llm.ep_world > 1:
+            raise ValueError("logprobs are single-GPU (the expert-parallel mode serves greedy requests)")
         if input_ids.shape[0] != 1:
             raise ValueError("generate() is single-sequence like the demo; use generate_batch() for more")
         emb, lens = self._embeds_for(input_ids, images, audios)
         llm = self.llm
         llm.check_capacity(lens[0], max_new_tokens)
         llm.reset()
-        llm.sampling.set(0, params)
+        llm.sampling.set(0, params, n_top)
+        width = llm.sampling.log_width(0, 1)                  # top entries the logprob log records (None: no log)
         score_log = llm.enable_score_log() if output_scores else None
+        if want_lp:
+            llm.enable_logprob_log()
         first = llm.prefill(emb[0, : lens[0]].contiguous(), slot=0, want_last_logits=output_scores, sampled=sampled,
-                            scores=score_log)
+                            scores=score_log, logprobs=width)
         if output_scores and not sampled:
             score_log[0].copy_(first[0])
         prompt = input_ids[0].tolist()
@@ -442,7 +463,8 @@ class VITAMixtralForCausalLM:
         while step < max_new_tokens and not done:
             n = min(sync_every, max_new_tokens - step)
             for _ in range(n):
-                llm.decode_step(1, use_graph=use_graph, want_logits=output_scores, sampled=sampled)
+                llm.decode_step(1, use_graph=use_graph, want_logits=output_scores, sampled=sampled,
+                                logprobs=width)
             step += n
             toks = llm.generated_tokens(0)[:max_new_tokens]     # one host sync per `sync_every` tokens
             n_new = len(toks)
@@ -461,4 +483,5 @@ class VITAMixtralForCausalLM:
         if not return_dict_in_generate:
             return seq
         scores = tuple(score_log[i: i + 1] for i in range(n_new)) if output_scores else None
-        return GenerateOutput(seq, scores)
+        lps = tuple(llm.read_logprobs(0, seq_host[0, L: L + n_new].tolist(), n_top)) if want_lp else None
+        return GenerateOutput(seq, scores, lps)

@@ -240,6 +240,52 @@ def sample_rows(logits, temperature, top_k, top_p, seed, counter, best, scores: 
               _p(seed), _p(counter), _p(best), _p(scores), V, rows, _stream())
 
 
+def sample_logprobs(logits, temperature, top_k, top_p, seed, counter, best, logprob, rank, top_ids, top_logprobs,
+                    n_top: int, target: Optional[torch.Tensor] = None, scores: Optional[torch.Tensor] = None):
+    """`sample_rows` plus log-probabilities over the processed row (contract: vita_b200/sampling.py).
+    `target` (i32 [B], optional): rows with target[b] in [0, V) score that token and draw nothing (best[b] gets the
+    greedy word); the other rows score the token they choose.  Outputs: logprob f32 / rank i32 of shape [B] (row b) or
+    [B, rows] (row counter[b] of request b, a device-resident log); top_ids i32 / top_logprobs f32 of that shape plus
+    a last dimension >= n_top (0 <= n_top <= 20): the n_top largest logits, lowest index first on ties."""
+    _chk(logits, BF16, "logits", contiguous=False); _chk(best, torch.int64, "best")
+    _chk(temperature, torch.float32, "temperature"); _chk(top_p, torch.float32, "top_p")
+    _chk(top_k, torch.int32, "top_k"); _chk(counter, torch.int32, "counter"); _chk(seed, torch.int64, "seed")
+    _chk(logprob, torch.float32, "logprob"); _chk(rank, torch.int32, "rank")
+    B, V = logits.shape
+    if logits.stride(1) != 1:
+        raise _lib.VitaB200Error("sample_logprobs: logits rows must be contiguous")
+    for t, n in ((temperature, "temperature"), (top_k, "top_k"), (top_p, "top_p"), (seed, "seed"),
+                 (counter, "counter"), (best, "best"), (logprob, "logprob"), (rank, "rank")):
+        if t.shape[0] < B:
+            raise _lib.VitaB200Error(f"sample_logprobs: {n} has fewer than {B} rows")
+    if logprob.shape != rank.shape or logprob.dim() not in (1, 2):
+        raise _lib.VitaB200Error("sample_logprobs: logprob and rank must both be [B] or [B, rows]")
+    out_rows = logprob.shape[1] if logprob.dim() == 2 else 0
+    top_ld = 0
+    if n_top > 0:
+        _chk(top_ids, torch.int32, "top_ids"); _chk(top_logprobs, torch.float32, "top_logprobs")
+        if top_ids.shape != top_logprobs.shape or tuple(top_ids.shape[:-1]) != tuple(logprob.shape) \
+                or top_ids.shape[-1] < n_top:
+            raise _lib.VitaB200Error("sample_logprobs: top_ids / top_logprobs must be logprob's shape + [>= n_top]")
+        top_ld = top_ids.shape[-1]
+    if target is not None:
+        _chk(target, torch.int32, "target")
+        if target.numel() < B:
+            raise _lib.VitaB200Error(f"sample_logprobs: target has fewer than {B} rows")
+    rows = 0
+    if scores is not None:
+        _chk(scores, BF16, "scores")
+        if scores.dim() == 2:
+            scores = scores.unsqueeze(0)
+        if scores.shape[0] < B or scores.shape[2] != V:
+            raise _lib.VitaB200Error("sample_logprobs: scores must be [B, rows, V]")
+        rows = scores.shape[1]
+    _lib.call("vita_sample_rows_logprobs", _p(logits), logits.stride(0), B, V, _p(temperature), _p(top_k), _p(top_p),
+              _p(seed), _p(counter), _p(target), _p(best), _p(scores), V, rows, _p(logprob), _p(rank),
+              _p(top_ids) if n_top > 0 else None, _p(top_logprobs) if n_top > 0 else None, int(n_top), top_ld,
+              out_rows, _stream())
+
+
 # ------------------------------------------------------------------------------------------------ MoE (prefill)
 def moe_router(h, norm_w, gate_w, xn, topk_ids, topk_w, eps):
     _chk(h, BF16, "h"); _chk(norm_w, BF16, "norm_w"); _chk(gate_w, BF16, "gate_w"); _chk(xn, BF16, "xn")

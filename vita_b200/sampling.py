@@ -14,11 +14,26 @@ of HF and vLLM, not their torch RNG streams.
 Parameters come from two surfaces:
   * HF `generate(do_sample=True, temperature=, top_k=, top_p=, seed=)` -> `from_hf`;
   * vLLM `SamplingParams` (per sequence group) -> `from_vllm`.
+
+Log-probabilities (`ops.sample_logprobs`; `generate(logprobs=N)`, `Request.logprobs`, the vLLM adapter's
+`sample_with_logprobs`).  For a row with parameters (T, top_k, top_p) the processed row is the bf16 logits as fp32
+when T = 0 (greedy), and otherwise x = l / T over the kept set of the warp above and -inf outside it: the row the score
+log holds and the token was chosen from.
+  * logprob(r) = x_r - logsumexp(processed row), -inf outside the kept set: HF's
+    `compute_transition_scores(sequences, scores, normalize_logits=True)` over this library's scores, and vLLM 0.5.5's
+    Sampler (one log_softmax over the processed logits, for sampled and prompt rows alike);
+  * rank(r) = 1 + #{tokens with a strictly greater processed value} (vLLM's `Logprob.rank`);
+  * top-N (0 <= N <= 20, vLLM's default `max_logprobs`): the N tokens ordered by (logit descending, index ascending)
+    with their logprobs; ids are compared on the bf16 logits, so they are exact;
+  * the log-sum-exp is fp32 with Z = sum of the fixed-point masses exp(x - x_max) * 2^40 as u64 integers, like the
+    top-p pass: independent of summation order and of batch position.
+A row with a target token (vLLM prompt-logprob rows: the next prompt token) is scored with its parameters and nothing
+is drawn.
 """
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import List, Optional
+from typing import List, Optional, Tuple
 
 import torch
 
@@ -27,6 +42,8 @@ HF_DEFAULT_TEMPERATURE, HF_DEFAULT_TOP_K, HF_DEFAULT_TOP_P = 1.0, 50, 1.0
 # vLLM samples when temperature >= _SAMPLING_EPS (vllm/sampling_params.py); below it the request is greedy
 VLLM_SAMPLING_EPS = 1e-5
 U64 = (1 << 64) - 1
+# most top-N entries a row can return (vLLM 0.5.5's default max_logprobs)
+MAX_LOGPROBS = 20
 
 # sampling-only kwargs of HF generate() this library does not implement: name -> value that leaves the output as is
 _HF_UNSUPPORTED = {"typical_p": 1.0, "min_p": None, "epsilon_cutoff": 0.0, "eta_cutoff": 0.0,
@@ -50,6 +67,34 @@ class SamplingParams:
             raise ValueError(f"top_p must be in [0, 1], got {self.top_p}")
         if not 0 <= self.seed <= U64:
             raise ValueError(f"seed must be in [0, 2**64), got {self.seed}")
+
+
+@dataclass(frozen=True)
+class TokenLogprobs:
+    """Log-probability record of one token: its id, logprob and rank over the processed row, and the top-N as
+    (id, logprob) pairs, highest logit first."""
+    token: int
+    logprob: float
+    rank: int
+    top: Tuple[Tuple[int, float], ...] = ()
+
+
+def check_logprobs(n, name: str = "logprobs") -> Optional[int]:
+    """A requested top-N count: None (no logprobs) or an int in [0, MAX_LOGPROBS]; anything else raises ValueError."""
+    if n is None:
+        return None
+    if isinstance(n, bool) or not isinstance(n, int):
+        raise ValueError(f"`{name}` must be an int in [0, {MAX_LOGPROBS}] or None, got {n!r}")
+    if not 0 <= n <= MAX_LOGPROBS:
+        raise ValueError(f"`{name}` must be in [0, {MAX_LOGPROBS}], got {n}")
+    return n
+
+
+def logprob_records(tokens, logprob, rank, top_ids, top_logprobs, n_top: int) -> List[TokenLogprobs]:
+    """Host records from the kernel's outputs (row i of each array belongs to tokens[i]; n_top <= their width)."""
+    lp, rk = logprob.tolist(), rank.tolist()
+    ti, tl = top_ids[:, :n_top].tolist(), top_logprobs[:, :n_top].tolist()
+    return [TokenLogprobs(int(t), lp[i], rk[i], tuple(zip(ti[i], tl[i]))) for i, t in enumerate(tokens)]
 
 
 def draw_key(generator: Optional[torch.Generator] = None) -> int:
@@ -83,10 +128,11 @@ def from_hf(do_sample: bool, temperature=None, top_k=None, top_p=None, seed: Opt
     return SamplingParams(float(t), int(k), p, draw_key() if seed is None else int(seed))
 
 
-def from_vllm(sp) -> Optional[SamplingParams]:
+def from_vllm(sp, draws: bool = True) -> Optional[SamplingParams]:
     """vLLM SamplingParams -> SamplingParams, or None for greedy (temperature < 1e-5).  top_k -1 or 0 is off.
-    Unseeded sampled rows get a fresh key from torch's default generator (call order = row order).  Features outside
-    this sampler raise NotImplementedError."""
+    Unseeded sampled rows get a fresh key from torch's default generator (call order = row order); with `draws` False
+    (rows that are only scored, e.g. prompt-logprob rows) they get key 0 and the generator does not advance.  Features
+    outside this sampler raise NotImplementedError."""
     g = lambda name, default: getattr(sp, name, default)
     if g("n", 1) > 1 or (g("best_of", None) or 1) > 1:
         raise NotImplementedError("n > 1 / best_of > 1 (several sequences per request) is not supported")
@@ -103,7 +149,8 @@ def from_vllm(sp) -> Optional[SamplingParams]:
     if k < -1:
         raise ValueError(f"top_k must be -1 (disable) or at least 1, got {k}")
     seed = g("seed", None)
-    return SamplingParams(t, max(k, 0), float(g("top_p", 1.0)), draw_key() if seed is None else int(seed) & U64)
+    key = (draw_key() if draws else 0) if seed is None else int(seed) & U64
+    return SamplingParams(t, max(k, 0), float(g("top_p", 1.0)), key)
 
 
 def _i64(u: int) -> int:
@@ -133,13 +180,15 @@ class SlotSampling:
         self.top_p = torch.ones(max_batch, dtype=torch.float32, device=dev)
         self.seed = torch.zeros(max_batch, dtype=torch.int64, device=dev)
         self.sampled: List[bool] = [False] * max_batch
+        self.logprobs: List[Optional[int]] = [None] * max_batch     # top-N a slot's request asked for (None: none)
 
     @property
     def tensors(self):
         return [self.temperature, self.top_k, self.top_p, self.seed]
 
-    def set(self, slot: int, params: Optional[SamplingParams]) -> None:
-        """params None = greedy."""
+    def set(self, slot: int, params: Optional[SamplingParams], logprobs: Optional[int] = None) -> None:
+        """params None = greedy; `logprobs` = the request's top-N (None: no logprobs)."""
+        self.logprobs[slot] = check_logprobs(logprobs)
         p = params or SamplingParams(1.0)
         row = slice(slot, slot + 1)
         self.temperature[row] = p.temperature if params is not None else 0.0
@@ -150,6 +199,15 @@ class SlotSampling:
 
     def swap(self, i: int, j: int) -> None:
         self.sampled[i], self.sampled[j] = self.sampled[j], self.sampled[i]
+        self.logprobs[i], self.logprobs[j] = self.logprobs[j], self.logprobs[i]
 
     def any_sampled(self, n: int) -> bool:
         return any(self.sampled[:n])
+
+    def log_width(self, s0: int, n: int) -> Optional[int]:
+        """Top entries a step over slots [s0, s0 + n) records: None (no slot asks for logprobs), 0 (only logprob and
+        rank: no slot asks for top entries) or MAX_LOGPROBS."""
+        asked = [x for x in self.logprobs[s0:s0 + n] if x is not None]
+        if not asked:
+            return None
+        return MAX_LOGPROBS if any(asked) else 0

@@ -3,7 +3,8 @@
 Mirrors `MixtralForConditionalGeneration` of the reference's vLLM fork
 (web_demo/vllm_tools/vllm_file/mixtral.py:897-1330): `forward` over FLATTENED tokens with the engine's paged KV cache
 (:1130-1172), `merge_multimodal_embeddings` (:1084-1128, placeholder ids -> feature rows, in place), `compute_logits`
-(:1174-1178), `sample` (:1180-1186; greedy or sampled per sequence group) and `load_weights` with the checkpoint -> kernel name map (:1189-1330).
+(:1174-1178), `sample` (:1180-1186; greedy or sampled per sequence group; `sample_with_logprobs` adds the logprobs
+vLLM's Sampler returns: chosen token, top-N and prompt logprobs) and `load_weights` with the checkpoint -> kernel name map (:1189-1330).
 
 What the engine hands the model per step is captured by `TokenBatch` (the fields of vLLM's flash-attention metadata:
 slot mapping, block tables, sequence / query lengths); the engine's block tables and KV tensors are used as they are --
@@ -21,14 +22,14 @@ exercised without a live engine on a GPU, so the tested contract is the call seq
 """
 from __future__ import annotations
 
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 from typing import Iterable, List, Optional, Sequence, Tuple
 
 import torch
 
 from . import ops, weights as W
 from .config import VitaConfig
-from .sampling import from_vllm, row_tensors
+from .sampling import TokenLogprobs, check_logprobs, from_vllm, logprob_records, row_tensors
 from .model.internvit import InternViTVisionTower, VisionProjector
 from .model.mixtral import LayerAttention, MixtralDecoder
 from .model.whale import AudioEncoder
@@ -53,6 +54,15 @@ class TokenBatch:
         if bt is None:
             bt = md.block_tables
         return TokenBatch(md.slot_mapping.to(torch.int32), bt.to(torch.int32), qsl, sl)
+
+
+@dataclass
+class GroupLogprobs:
+    """Logprobs of one sequence group (vLLM 0.5.5's SamplerOutput fields): `sample` for the token it sampled (logprob,
+    rank, top-`SamplingParams.logprobs`), `prompt` for its prompt-logprob rows in order (each scores the next prompt
+    token, with top-`SamplingParams.prompt_logprobs`)."""
+    sample: Optional[TokenLogprobs] = None
+    prompt: List[TokenLogprobs] = field(default_factory=list)
 
 
 class MixtralForConditionalGeneration:
@@ -212,7 +222,17 @@ class MixtralForConditionalGeneration:
         if groups is None:
             ops.argmax_rows(logits.contiguous(), best)
             return (0xFFFFFFFF - (best & 0xFFFFFFFF)).to(torch.int64)
-        params, counter = [None] * B, [0] * B
+        params, counter, _ = self._sampled_rows(groups, B)
+        T, K, P, S = row_tensors(params, logits.device)
+        cnt = torch.tensor(counter, dtype=torch.int32).to(logits.device, non_blocking=True)
+        ops.sample_rows(logits.contiguous(), T, K, P, S, cnt, best)
+        return (0xFFFFFFFF - (best & 0xFFFFFFFF)).to(torch.int64)
+
+    @staticmethod
+    def _sampled_rows(groups, B: int):
+        """-> per-row SamplingParams (None = greedy) and counters of the rows the groups sample, and per group its
+        sampled row (or None) with its parameters."""
+        params, counter, sampled = [None] * B, [0] * B, [None] * len(groups)
         for i, sg in enumerate(groups):
             if not getattr(sg, "do_sample", True):
                 continue
@@ -231,10 +251,73 @@ class MixtralForConditionalGeneration:
                 raise ValueError(f"sample index {rows[0]} outside the {B} logits rows")
             params[rows[0]] = from_vllm(sg.sampling_params)
             counter[rows[0]] = int(sg.seq_data[ids[0]].get_output_len())
-        T, K, P, S = row_tensors(params, logits.device)
-        cnt = torch.tensor(counter, dtype=torch.int32).to(logits.device, non_blocking=True)
-        ops.sample_rows(logits.contiguous(), T, K, P, S, cnt, best)
-        return (0xFFFFFFFF - (best & 0xFFFFFFFF)).to(torch.int64)
+            sampled[i] = (rows[0], params[rows[0]])
+        return params, counter, sampled
+
+    @torch.no_grad()
+    def sample_with_logprobs(self, logits: torch.Tensor, sampling_metadata):
+        """`sample()` plus the logprobs of vLLM 0.5.5's Sampler: -> (ids [B] as `sample()` returns them, one
+        GroupLogprobs per sequence group).  A group that samples gets its token's logprob and rank over the processed
+        row (vita_b200/sampling.py) with the top-`sampling_params.logprobs`.  With `sampling_params.prompt_logprobs`
+        set, its `prompt_logprob_indices` rows score the next prompt token -- row j of a chunk that starts after
+        `seq_data.get_num_computed_tokens()` tokens scores prompt token computed + j + 1 -- with the group's
+        parameters, chunked-prefill chunks included.  One kernel launch for all rows."""
+        B = logits.shape[0]
+        groups = getattr(sampling_metadata, "seq_groups", None)
+        if groups is None:
+            raise ValueError("sample_with_logprobs needs SamplingMetadata with seq_groups")
+        params, counter, sampled = self._sampled_rows(groups, B)
+        target = [-1] * B
+        used = {g[0] for g in sampled if g is not None}        # every row belongs to at most one group
+        n_top, prompt_rows = 0, [None] * len(groups)
+        for i, sg in enumerate(groups):
+            sp = sg.sampling_params
+            n = check_logprobs(getattr(sp, "logprobs", None), "logprobs")
+            if sampled[i] is not None:
+                n_top = max(n_top, n or 0)
+            n_prompt = check_logprobs(getattr(sp, "prompt_logprobs", None), "prompt_logprobs")
+            rows = [int(r) for r in (getattr(sg, "prompt_logprob_indices", None) or [])]
+            if n_prompt is None or not rows:
+                continue
+            data = sg.seq_data[list(sg.seq_ids)[0]]
+            prompt, done = list(data.prompt_token_ids), int(data.get_num_computed_tokens())
+            if done + len(rows) >= len(prompt):
+                raise ValueError(f"{len(rows)} prompt-logprob rows after {done} computed tokens of a "
+                                 f"{len(prompt)}-token prompt")
+            # the group's parameters; a scoring row draws nothing, so it never takes a key from torch's generator
+            p = sampled[i][1] if sampled[i] is not None else from_vllm(sp, draws=False)
+            for j, r in enumerate(rows):
+                if not 0 <= r < B or r in used:
+                    raise ValueError(f"prompt-logprob row {r} is outside the {B} logits rows or used twice")
+                used.add(r)
+                params[r], target[r] = p, prompt[done + 1 + j]
+            prompt_rows[i] = (rows, n_prompt)
+            n_top = max(n_top, n_prompt)
+        dev = logits.device
+        T, K, P, S = row_tensors(params, dev)
+        cnt = torch.tensor(counter, dtype=torch.int32).to(dev, non_blocking=True)
+        tgt = torch.tensor(target, dtype=torch.int32).to(dev, non_blocking=True)
+        best = torch.zeros(B, dtype=torch.int64, device=dev)
+        lp = torch.empty(B, dtype=torch.float32, device=dev)
+        rank = torch.empty(B, dtype=torch.int32, device=dev)
+        top_ids = torch.empty(B, max(n_top, 1), dtype=torch.int32, device=dev)
+        top_lp = torch.empty(B, max(n_top, 1), dtype=torch.float32, device=dev)
+        ops.sample_logprobs(logits.contiguous(), T, K, P, S, cnt, best, lp, rank, top_ids, top_lp, n_top, target=tgt)
+        ids = (0xFFFFFFFF - (best & 0xFFFFFFFF)).to(torch.int64)
+        toks = [t if t >= 0 else w for t, w in zip(target, ids.tolist())]
+        lp, rank, top_ids, top_lp = lp.cpu(), rank.cpu(), top_ids.cpu(), top_lp.cpu()
+        rec = lambda rows, n: logprob_records([toks[r] for r in rows], lp[rows], rank[rows], top_ids[rows],
+                                              top_lp[rows], n)
+        out = []
+        for i, sg in enumerate(groups):
+            g = GroupLogprobs()
+            if sampled[i] is not None:
+                n = check_logprobs(getattr(sg.sampling_params, "logprobs", None)) or 0
+                g.sample = rec([sampled[i][0]], n)[0]
+            if prompt_rows[i] is not None:
+                g.prompt = rec(*prompt_rows[i])
+            out.append(g)
+        return ids, out
 
 
 def register() -> bool:
