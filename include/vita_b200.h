@@ -280,6 +280,23 @@ int vita_sample_rows_logprobs(const void* logits, int64_t ld, int64_t B, int64_t
                               const int32_t* target, uint64_t* best, void* scores, int64_t score_ld,
                               int64_t score_rows, float* logprob, int32_t* rank, int32_t* top_ids,
                               float* top_logprobs, int64_t n_top, int64_t top_ld, int64_t out_rows, void* stream);
+/* vita_sample_rows_logprobs whose score rows receive the processed row's log-softmax instead: bf16(logprob(r)) of
+ * every token, logprob(r) = x_r - x_max - log Z from the same Z as the logprob outputs (-inf outside the kept set).
+ * HF beam search's per-step scores (the running beams' log-softmax rows). */
+int vita_sample_rows_logsoftmax(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
+                                const int32_t* top_k, const float* top_p, const uint64_t* seed,
+                                const int32_t* counter, const int32_t* target, uint64_t* best, void* scores,
+                                int64_t score_ld, int64_t score_rows, float* logprob, int32_t* rank, int32_t* top_ids,
+                                float* top_logprobs, int64_t n_top, int64_t top_ld, int64_t out_rows, void* stream);
+/* Copy-on-write of the paged KV cache (vLLM's copy_blocks): for every (src, dst) page pair of pairs [n_pairs, 2] i32
+ * (device) and every cache of layer_base [n_bases] (device pointers: the K and the V cache of each layer, each
+ * n_pages pages of page_bytes bytes, 16-byte aligned), copy page src over page dst.  One launch, 16-byte vector
+ * copies, bit-exact; pairs with an index outside [0, n_pages) are skipped.  The pairs of one launch run concurrently:
+ * no dst page may also be a src page of the launch, and no two pairs may share a dst page (beam search's PagePool
+ * takes every dst fresh from its free list and copies only pages that are still referenced).  Beam search forks a
+ * sequence's cache with it. */
+int vita_kv_copy_pages(const uint64_t* layer_base, int64_t n_bases, const int32_t* pairs, int64_t n_pairs,
+                       int64_t n_pages, int64_t page_bytes, void* stream);
 /* ---- greedy decode step on the tensor cores (wgmma swap-AB GEMV, stream-K) ---------------------------------
  * Every linear of the decode step as a weight-streaming GEMV on the tensor cores: the weight tile is the M operand of
  * wgmma and the activation vector as row 0 of a 16-wide N operand; (row-block, k-block) units are split evenly

@@ -20,6 +20,8 @@
 //   ties (the N-th largest comes from the same radix selection as top-k, with k = N).  Both compare the ordered keys
 //   with -0.0 read as +0.0, so equal logits are equal.
 // A row with a target id scores that token and draws nothing (prompt rows: the next prompt token).
+// The LSM variant (vita_sample_rows_logsoftmax) writes bf16(logprob(r)) of every token to the score row instead of the
+// processed row: HF beam search's per-step scores, from the same Z as the logprob.
 //
 // Reference call sites: vLLM's Sampler (web_demo/vllm_tools/vllm_file/mixtral.py:1180-1186) and the sampling loop of
 // HF generate() (video_audio_demo.py:257-270: TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper ->
@@ -210,11 +212,13 @@ __device__ __forceinline__ float key_x(uint32_t k, float T) {
 }
 
 // Logprob, rank and top-N of token `idx` over the processed row (kept set = keys >= thr).  Every thread calls it.
-template <bool SCALED>
+// LSM: srow (may be null) receives the log-softmax of the whole processed row.
+template <bool SCALED, bool LSM>
 __device__ void write_logprobs(const uint16_t* keys, int V, uint32_t thr, float T, float x_max, int idx,
                                             int n, int b, const LogprobArgs& lp, unsigned long long* whist,
                                             unsigned long long* tot, unsigned long long* red, int* s_bin,
-                                            unsigned long long* s_above, unsigned long long* s_total) {
+                                            unsigned long long* s_above, unsigned long long* s_total,
+                                            __nv_bfloat16* srow) {
     __shared__ int s_top[kMaxTopLogprobs];
     __shared__ int s_cnt, s_wcnt[kSampleWarps];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -231,6 +235,10 @@ __device__ void write_logprobs(const uint16_t* keys, int V, uint32_t thr, float 
     gt = block_sum_u64(gt, red);
     const float log_z = logf(__ull2float_rn(z) * 0x1p-40f);
     auto logprob_of = [&](uint32_t k) { return k >= thr ? (key_x<SCALED>(k, T) - x_max) - log_z : -INFINITY; };
+    if constexpr (LSM) {
+        if (srow != nullptr)
+            for (int i = tid; i < V; i += kSampleThreads) srow[i] = __float2bfloat16(logprob_of(keys[i]));
+    }
 
     long long row = b;
     if (lp.rows > 0) {
@@ -291,7 +299,7 @@ __device__ void write_logprobs(const uint16_t* keys, int V, uint32_t thr, float 
     }
 }
 
-template <bool LOGPROBS>
+template <bool LOGPROBS, bool LSM = false>
 __global__ void __launch_bounds__(kSampleThreads, 1)
 sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, const float* __restrict__ temperature,
                    const int* __restrict__ top_k, const float* __restrict__ top_p,
@@ -358,7 +366,7 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
 
     if (greedy) {                                        // bit-identical to argmax_rows; the score log gets the logits
         if (tid == 0) best[b] = arg;
-        if (srow != nullptr)
+        if (srow != nullptr && !LSM)
             for (int i = tid; i < V; i += kSampleThreads) srow[i] = __float2bfloat16(key_value(keys[i]));
         if constexpr (!LOGPROBS) return;
     }
@@ -367,8 +375,8 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
     if constexpr (LOGPROBS) {
         if (greedy) {                                    // the processed row is the logits: x = l, every token kept
             const int idx = tgt >= 0 ? tgt : static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(arg & 0xFFFFFFFFull));
-            write_logprobs<false>(keys, V, 0u, 1.0f, key_value(max_key), idx, n, b, lp, whist, tot, red, &s_bin,
-                                  &s_above, &s_total);
+            write_logprobs<false, LSM>(keys, V, 0u, 1.0f, key_value(max_key), idx, n, b, lp, whist, tot, red, &s_bin,
+                                       &s_above, &s_total, srow);
             return;
         }
     }
@@ -446,7 +454,8 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
     if constexpr (LOGPROBS) {
         if (tgt >= 0) {                                  // a scored row leaves the greedy word in best
             if (tid == 0) best[b] = arg;
-            write_logprobs<true>(keys, V, thr, T, x_max, tgt, n, b, lp, whist, tot, red, &s_bin, &s_above, &s_total);
+            write_logprobs<true, LSM>(keys, V, thr, T, x_max, tgt, n, b, lp, whist, tot, red, &s_bin, &s_above,
+                                      &s_total, srow);
             return;
         }
     }
@@ -456,9 +465,9 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
         best[b] = pack_score(key_value(keys[idx]), idx);
     }
     if constexpr (LOGPROBS)
-        write_logprobs<true>(keys, V, thr, T, x_max,
-                             static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(win & 0xFFFFFFFFull)), n, b, lp,
-                             whist, tot, red, &s_bin, &s_above, &s_total);
+        write_logprobs<true, LSM>(keys, V, thr, T, x_max,
+                                  static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(win & 0xFFFFFFFFull)), n, b, lp,
+                                  whist, tot, red, &s_bin, &s_above, &s_total, srow);
 }
 
 }  // namespace vita
@@ -467,7 +476,7 @@ using namespace vita;
 
 namespace {
 
-template <bool LOGPROBS>
+template <bool LOGPROBS, bool LSM = false>
 int launch_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
                        const int32_t* top_k, const float* top_p, const uint64_t* seed, const int32_t* counter,
                        uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows, const LogprobArgs& lp,
@@ -484,7 +493,7 @@ int launch_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, con
         cudaFuncAttributes fa{};
         int rc = check_cuda(cudaGetDevice(&dev), "sample_rows");
         if (!rc) rc = check_cuda(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev), "sample_rows");
-        if (!rc) rc = check_cuda(cudaFuncGetAttributes(&fa, sample_rows_kernel<LOGPROBS>), "sample_rows");
+        if (!rc) rc = check_cuda(cudaFuncGetAttributes(&fa, sample_rows_kernel<LOGPROBS, LSM>), "sample_rows");
         if (rc) return rc;
         dyn_limit = static_cast<size_t>(optin) > fa.sharedSizeBytes ? static_cast<size_t>(optin) - fa.sharedSizeBytes : 0;
     }
@@ -494,7 +503,7 @@ int launch_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, con
                                         " on this device)");
     static size_t configured = 0;
     if (smem > configured) {
-        const int rc = check_cuda(cudaFuncSetAttribute(sample_rows_kernel<LOGPROBS>,
+        const int rc = check_cuda(cudaFuncSetAttribute(sample_rows_kernel<LOGPROBS, LSM>,
                                                        cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                        static_cast<int>(smem)), "sample_rows");
         if (rc) return rc;
@@ -503,13 +512,28 @@ int launch_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, con
     const int vec = (V % 8 == 0 && ld % 8 == 0 && aligned16(logits)) ? 1 : 0;
     // launched as a programmatic dependent of the LM head: the kernel waits (griddepcontrol.wait) before reading the
     // logits and never triggers its own dependents early, so the next step starts after its last write of `best`
-    cudaError_t e = launch_chain(sample_rows_kernel<LOGPROBS>, dim3(static_cast<unsigned>(B)), dim3(kSampleThreads), smem,
+    cudaError_t e = launch_chain(sample_rows_kernel<LOGPROBS, LSM>, dim3(static_cast<unsigned>(B)), dim3(kSampleThreads), smem,
                                  static_cast<cudaStream_t>(stream), BF16C(logits), (long long)ld, (int)V, temperature,
                                  top_k, top_p, reinterpret_cast<const unsigned long long*>(seed), counter,
                                  reinterpret_cast<unsigned long long*>(best), static_cast<__nv_bfloat16*>(scores),
                                  (long long)score_ld, (int)score_rows, vec, lp);
     if (e != cudaSuccess) return check_cuda(e, "sample_rows");
     return check_launch("sample_rows");
+}
+
+template <bool LSM>
+int launch_logprobs(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
+                    const int32_t* top_k, const float* top_p, const uint64_t* seed, const int32_t* counter,
+                    const int32_t* target, uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows,
+                    float* logprob, int32_t* rank, int32_t* top_ids, float* top_logprobs, int64_t n_top,
+                    int64_t top_ld, int64_t out_rows, void* stream) {
+    VITA_REQUIRE(logprob && rank, "logprob and rank outputs are required");
+    VITA_REQUIRE(n_top >= 0 && n_top <= kMaxTopLogprobs && n_top <= V, "need 0 <= n_top <= min(20, V)");
+    VITA_REQUIRE(n_top == 0 || (top_ids && top_logprobs && top_ld >= n_top), "top-N outputs: need top_ld >= n_top");
+    VITA_REQUIRE(out_rows >= 0, "out_rows must be >= 0");
+    const LogprobArgs lp{target, logprob, rank, top_ids, top_logprobs, (int)n_top, (int)top_ld, (int)out_rows};
+    return launch_sample_rows<true, LSM>(logits, ld, B, V, temperature, top_k, top_p, seed, counter, best, scores,
+                                         score_ld, score_rows, lp, stream);
 }
 
 }  // namespace
@@ -521,17 +545,23 @@ extern "C" int vita_sample_rows(const void* logits, int64_t ld, int64_t B, int64
                                      score_rows, LogprobArgs{}, stream);
 }
 
+#define VITA_LOGPROBS_ARGS logits, ld, B, V, temperature, top_k, top_p, seed, counter, target, best, scores, score_ld, \
+                           score_rows, logprob, rank, top_ids, top_logprobs, n_top, top_ld, out_rows, stream
+
 extern "C" int vita_sample_rows_logprobs(const void* logits, int64_t ld, int64_t B, int64_t V,
                                          const float* temperature, const int32_t* top_k, const float* top_p,
                                          const uint64_t* seed, const int32_t* counter, const int32_t* target,
                                          uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows,
                                          float* logprob, int32_t* rank, int32_t* top_ids, float* top_logprobs,
                                          int64_t n_top, int64_t top_ld, int64_t out_rows, void* stream) {
-    VITA_REQUIRE(logprob && rank, "logprob and rank outputs are required");
-    VITA_REQUIRE(n_top >= 0 && n_top <= kMaxTopLogprobs && n_top <= V, "need 0 <= n_top <= min(20, V)");
-    VITA_REQUIRE(n_top == 0 || (top_ids && top_logprobs && top_ld >= n_top), "top-N outputs: need top_ld >= n_top");
-    VITA_REQUIRE(out_rows >= 0, "out_rows must be >= 0");
-    const LogprobArgs lp{target, logprob, rank, top_ids, top_logprobs, (int)n_top, (int)top_ld, (int)out_rows};
-    return launch_sample_rows<true>(logits, ld, B, V, temperature, top_k, top_p, seed, counter, best, scores, score_ld,
-                                    score_rows, lp, stream);
+    return launch_logprobs<false>(VITA_LOGPROBS_ARGS);
+}
+
+extern "C" int vita_sample_rows_logsoftmax(const void* logits, int64_t ld, int64_t B, int64_t V,
+                                           const float* temperature, const int32_t* top_k, const float* top_p,
+                                           const uint64_t* seed, const int32_t* counter, const int32_t* target,
+                                           uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows,
+                                           float* logprob, int32_t* rank, int32_t* top_ids, float* top_logprobs,
+                                           int64_t n_top, int64_t top_ld, int64_t out_rows, void* stream) {
+    return launch_logprobs<true>(VITA_LOGPROBS_ARGS);
 }

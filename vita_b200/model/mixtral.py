@@ -20,8 +20,106 @@ from ..sampling import MAX_LOGPROBS, SlotSampling, logprob_records
 BF16 = torch.bfloat16
 
 
+class PagePool:
+    """Host page tables with reference counts: copy-on-write sharing of KV pages between sequences (beam search).
+
+    table[slot][i] is the page of positions [i * page_size, (i + 1) * page_size) of the slot, -1 for none.  At
+    construction and after reset() every slot owns its row of `static`, the table at rest (rebase() takes a new one).  A forked or reordered slot holds the
+    pages that cover its `length` tokens: full pages are shared (they are never written again), and the page its next
+    row lands in (index length // page_size) is private to it.  refs[page] counts the table entries that point to the
+    page; pages whose count drops to 0 go to `free` and are handed out again."""
+
+    def __init__(self, static: torch.Tensor, page_size: int):
+        self.static = static.to("cpu", torch.int32).clone()     # never a view of a device-side table
+        self.page_size = page_size
+        self.reset()
+
+    def rebase(self, static: torch.Tensor):
+        self.static = static.to("cpu", torch.int32).clone()
+        self.reset()
+
+    def reset(self):
+        self.table: List[List[int]] = self.static.tolist()
+        self.refs = [0] * self.static.numel()
+        for row in self.table:
+            for pg in row:
+                self.refs[pg] += 1
+        self.free: List[int] = []
+
+    def _drop(self, pg: int):
+        self.refs[pg] -= 1
+        if self.refs[pg] == 0:
+            self.free.append(pg)
+
+    def _private_write_pages(self, slots: Sequence[int], length: int) -> List[Tuple[int, int]]:
+        """Make page length // page_size of every slot private: a fresh page where there is none, a copy where it is
+        shared (the last slot that shares it keeps the original).  Returns the (src, dst) pages to copy."""
+        w, pairs = length // self.page_size, []
+        for s in slots:
+            pg = self.table[s][w]
+            if pg >= 0 and self.refs[pg] == 1:
+                continue
+            if not self.free:
+                raise RuntimeError("KV page pool exhausted")
+            new = self.free.pop()
+            self.refs[new] += 1
+            if pg >= 0:
+                pairs.append((pg, new))
+                self._drop(pg)
+            self.table[s][w] = new
+        return pairs
+
+    def fork(self, src: int, dsts: Sequence[int], length: int) -> List[Tuple[int, int]]:
+        """dsts continue the `length` tokens of src: they share its full pages and get a copy of its partial last
+        page.  The pages of the dst rows and src's pages past its tokens return to the pool."""
+        n_cover = -(-length // self.page_size)
+        assert src not in dsts and length < len(self.table[src]) * self.page_size
+        for i, pg in enumerate(self.table[src]):
+            if i >= n_cover and pg >= 0:
+                self._drop(pg)
+                self.table[src][i] = -1
+        for d in dsts:
+            for pg in self.table[d]:
+                if pg >= 0:
+                    self._drop(pg)
+            self.table[d] = list(self.table[src])
+            for pg in self.table[d]:
+                if pg >= 0:
+                    self.refs[pg] += 1
+        return self._private_write_pages([*dsts, src], length)     # src keeps its page
+
+    def reorder(self, parents: Sequence[int], length: int) -> List[Tuple[int, int]]:
+        """Slot i (i < len(parents)) continues slot parents[i], every slot holding `length` tokens: each takes its
+        parent's row, then the page the next row lands in is made private (one child keeps the parent's page)."""
+        rows = [list(self.table[p]) for p in parents]
+        for row in rows:
+            for pg in row:
+                if pg >= 0:
+                    self.refs[pg] += 1
+        for i, row in enumerate(rows):
+            for pg in self.table[i]:
+                if pg >= 0:
+                    self._drop(pg)
+            self.table[i] = row
+        return self._private_write_pages(range(len(parents)), length)
+
+    def check(self):
+        """Invariants: each count equals the number of table entries pointing to the page, free pages are exactly
+        those with count 0."""
+        count = [0] * len(self.refs)
+        for row in self.table:
+            for pg in row:
+                if pg >= 0:
+                    count[pg] += 1
+        assert count == self.refs, "reference counts do not match the tables"
+        assert sorted(self.free) == [pg for pg, c in enumerate(count) if c == 0], "free list does not match"
+
+
 class PagedKVCache:
-    """k/v per layer: [num_pages * page_size, n_kv_heads, head_dim] bf16; block_table [max_batch, pages_per_seq]."""
+    """k/v per layer: [num_pages * page_size, n_kv_heads, head_dim] bf16; block_table [max_batch, pages_per_seq].
+    slot_map is derived from block_table, and the serving engine swaps the rows of both together with their slots.
+    fork / reorder change block_table rows only; unshare() (and reset()) gives every slot its row from before the
+    first of them back, so the two agree again."""
 
     def __init__(self, cfg: LLMConfig, max_batch: int, max_seq_len: int, device, page_size: int = 16,
                  shuffle_pages: bool = False, storage=None):
@@ -42,6 +140,9 @@ class PagedKVCache:
             else torch.arange(n_pages)
         table = order.view(max_batch, self.pages_per_seq).to(torch.int32)
         self.block_table = table.to(device)
+        self.pool = PagePool(table, page_size)
+        self.shared = False                  # fork / reorder changed block_table since the pool's rebase
+        self._layer_base = None
         pos = torch.arange(self.max_seq_len)
         self.slot_map = (table[:, pos // page_size].to(torch.int64) * page_size + (pos % page_size)[None, :]) \
             .to(torch.int32).to(device)                                      # [max_batch, max_seq_len]
@@ -51,6 +152,42 @@ class PagedKVCache:
     def reset(self):
         self.cache_len.zero_()
         self.cur_pos.zero_()
+        self.unshare()
+
+    def _share(self):
+        """The first fork / reorder since the table was at rest: the pool starts from block_table's rows as they are
+        now (they follow slot_map's rows, which the serving engine may have swapped)."""
+        if not self.shared:
+            self.pool.rebase(self.block_table.cpu())
+            self.shared = True
+
+    def unshare(self):
+        """Give every slot back the block_table row it had before the first fork / reorder, and refill the pool."""
+        if self.shared:
+            self.pool.reset()
+            self.block_table.copy_(self.pool.static)
+            self.shared = False
+
+    def fork(self, src: int, dsts: Sequence[int], length: int):
+        """PagePool.fork on the device tables; the partial page is copied for the dsts in one kv_copy_pages launch."""
+        self._share()
+        self._apply(self.pool.fork(src, dsts, length))
+
+    def reorder(self, parents: Sequence[int], length: int):
+        """PagePool.reorder on the device tables, with one kv_copy_pages launch for the pages it copies."""
+        self._share()
+        self._apply(self.pool.reorder(parents, length))
+
+    def _apply(self, pairs):
+        self.block_table.copy_(torch.tensor(self.pool.table, dtype=torch.int32))
+        if not pairs:
+            return
+        if self._layer_base is None:
+            self._layer_base = torch.tensor([t.data_ptr() for t in self.k + self.v], dtype=torch.int64,
+                                            device=self.block_table.device)
+        row_bytes = self.k[0][0].numel() * self.k[0].element_size()
+        ops.kv_copy_pages(self._layer_base, torch.tensor(pairs, dtype=torch.int32).to(self.block_table.device),
+                          self.k[0].shape[0] // self.page_size, self.page_size * row_bytes)
 
 
 @dataclass
@@ -162,6 +299,7 @@ class MixtralDecoder:
         self._graphs = {}             # single-sequence decode step: captured CUDA graph per (B, want_logits[, sampled])
         self.scores_buf = None        # [max_new_tokens + 1, V] logits log of slot 0 (generate(output_scores=True))
         self.lp_log = None            # per-slot logprob log (enable_logprob_log)
+        self.beam_scores = None       # per-slot log-softmax log of beam search (enable_beam_score_log)
         self._bgraphs = {}            # batched decode step: captured CUDA graph per (batch size, sampled)
         self.d_slots = torch.zeros(B, dtype=torch.int32, device=dev)
         self._prefill_ws = {}
@@ -292,7 +430,7 @@ class MixtralDecoder:
     @torch.no_grad()
     def prefill(self, inputs_embeds: torch.Tensor, slot: int = 0, all_logits: bool = False,
                 want_last_logits: bool = False, sampled: bool = False, scores: Optional[torch.Tensor] = None,
-                start: int = 0, final: bool = True, logprobs: Optional[int] = None):
+                start: int = 0, final: bool = True, logprobs: Optional[int] = None, log_softmax_scores: bool = False):
         """One sequence: inputs_embeds [S, H] bf16 (consumed as the residual stream, modified in place).
 
         Appends S tokens to the KV cache of batch slot `slot` (which must be empty), leaves the arg-max of the last
@@ -305,7 +443,8 @@ class MixtralDecoder:
         Chunked prefill / prefix reuse: `start` is the number of tokens the slot already holds (rows get positions
         start + i and attend the cached ones through the paged-KV attention kernel).  With `final` False the rows are
         only appended: no LM head, and best / the sampler counter are left alone; the last chunk of a prompt passes
-        `final` True and yields the first token as a whole-prompt prefill does."""
+        `final` True and yields the first token as a whole-prompt prefill does.
+        `log_softmax_scores` (with `logprobs` and `scores`): the score row is the log-softmax row (beam search)."""
         c, w = self.cfg, self.w
         S, H = inputs_embeds.shape
         assert inputs_embeds.dtype == BF16 and inputs_embeds.is_cuda and inputs_embeds.is_contiguous()
@@ -339,7 +478,7 @@ class MixtralDecoder:
         ops.tc_lm_head_argmax(h[S - 1:], H, w["norm"], w["lm_head"], last_logits, self.best[slot:slot + 1], 1,
                               self.tc_ws, c.rms_norm_eps)
         if sampled or logprobs is not None:
-            self._sample(slot, 1, scores, logprobs)
+            self._sample(slot, 1, scores, logprobs, log_softmax_scores)
         if all_logits:
             return ops.linear(xn, w["lm_head"])      # [S, V]; xn = final RMSNorm(h) written by the last combine
         return last_logits
@@ -465,10 +604,12 @@ class MixtralDecoder:
         else:
             self._log_scores(B, want_logits)
 
-    def _sample(self, s0: int, n: int, scores: Optional[torch.Tensor], logprobs: Optional[int] = None):
+    def _sample(self, s0: int, n: int, scores: Optional[torch.Tensor], logprobs: Optional[int] = None,
+                log_softmax_scores: bool = False):
         """Draw the next token of slots [s0, s0 + n) from d_logits into best (counter = gen_count of the slot).
         `logprobs` (the log width, SlotSampling.log_width: 0 or 20): also write the token's logprob, rank and that
-        many top entries at row gen_count of each slot's logprob log."""
+        many top entries at row gen_count of each slot's logprob log; `log_softmax_scores`: the score rows get the
+        log-softmax of the processed row."""
         sp, rows = self.sampling, slice(s0, s0 + n)
         if logprobs is None:
             ops.sample_rows(self.d_logits[rows], sp.temperature[rows], sp.top_k[rows], sp.top_p[rows], sp.seed[rows],
@@ -477,7 +618,7 @@ class MixtralDecoder:
         lg = self.enable_logprob_log()
         ops.sample_logprobs(self.d_logits[rows], sp.temperature[rows], sp.top_k[rows], sp.top_p[rows], sp.seed[rows],
                             self.gen_count[rows], self.best[rows], lg[0][rows], lg[1][rows], lg[2][rows], lg[3][rows],
-                            logprobs, scores=scores)
+                            logprobs, scores=scores, log_softmax_scores=log_softmax_scores)
 
     def enable_logprob_log(self):
         """Allocate the per-slot logprob log: (logprob f32 [B, R], rank i32 [B, R], top ids i32 [B, R, 20], top
@@ -498,6 +639,29 @@ class MixtralDecoder:
         holds them; the token log only receives a token when the next step consumes it), top-n_top each."""
         lp, rk, ti, tl = (t[slot, :len(tokens)].cpu() for t in self.lp_log)
         return logprob_records(tokens, lp, rk, ti, tl, n_top)
+
+    def enable_beam_score_log(self, n: int, rows: int) -> torch.Tensor:
+        """The per-slot log-softmax log of beam search's `output_scores`: [>= n, >= rows, V] bf16, row i of slot b
+        written by the step that produced token i (row index = gen_count).  Sized to the largest call so far (n beams,
+        `rows` = its max_new_tokens) and kept with the decoder; the batched-step graphs that write it are re-captured
+        when it grows."""
+        old = self.beam_scores
+        if old is None or old.shape[0] < n or old.shape[1] < rows:
+            n, rows = (n, rows) if old is None else (max(n, old.shape[0]), max(rows, old.shape[1]))
+            self.beam_scores = None
+            with torch.inference_mode(False):
+                self.beam_scores = torch.zeros(n, rows, self.cfg.vocab_size, dtype=BF16, device=self.device)
+            self._bgraphs = {k: g for k, g in self._bgraphs.items() if "scores" not in k}
+        return self.beam_scores
+
+    def fork(self, src: int, dsts: Sequence[int], length: int):
+        """Slots dsts continue slot src, which holds `length` tokens: its KV pages are shared copy-on-write
+        (PagedKVCache.fork) and its decode state (cache_len, cur_pos, gen_count, token log, next token) is copied."""
+        c = self.cache
+        idx = torch.tensor(list(dsts), dtype=torch.int64, device=self.device)
+        for t in (c.cache_len, c.cur_pos, self.gen_count, self.token_log, self.best):
+            t[idx] = t[src].clone()
+        c.fork(src, dsts, length)
 
     def enable_score_log(self):
         """Allocate the per-step logits log (HF `output_scores=True`): row i holds the logits token i was chosen from.
@@ -543,10 +707,12 @@ class MixtralDecoder:
         self._replay(self._graphs, key, step)
 
     # ------------------------------------------------------------------------------------------ batched decode
-    def _batched_step_kernels(self, B: int, sampled: bool = False, logprobs: Optional[int] = None):
+    def _batched_step_kernels(self, B: int, sampled: bool = False, logprobs: Optional[int] = None,
+                              scores: bool = False):
         """One token for each of B sequences through the GEMM path (weights of every touched expert are streamed once
         for the whole batch; BASELINE configs[4]).  The prefill's layer loop with M = B rows at B different
-        positions and the paged decode attention."""
+        positions and the paged decode attention.  `scores` (with `logprobs`): the sampler also writes each slot's
+        log-softmax row to the beam score log."""
         c, w, cache = self.cfg, self.w, self.cache
         h = self.d_h[:B]
         ops.decode_embed(self.best[:B], self.token_log[:B], self.gen_count[:B], cache.cache_len[:B], cache.cur_pos[:B],
@@ -558,7 +724,7 @@ class MixtralDecoder:
         xn = self.run_layers(h, cache.cur_pos[:B], slots, cache.k, cache.v, attention, final_norm=True)
         logits = ops.linear(xn, w["lm_head"], out=self.d_logits[:B])
         if sampled or logprobs is not None:   # greedy rows (temperature 0) get argmax_rows' word: a mixed batch keeps their tokens
-            self._sample(0, B, None, logprobs)
+            self._sample(0, B, self.beam_scores if scores else None, logprobs, scores)
         else:
             ops.argmax_rows(logits, self.best[:B])
 
@@ -568,13 +734,17 @@ class MixtralDecoder:
 
     @torch.no_grad()
     def decode_step_batched(self, B: int, use_graph: bool = True, sampled: bool = False,
-                            logprobs: Optional[int] = None):
+                            logprobs: Optional[int] = None, scores: bool = False):
+        """`scores`: write the log-softmax rows to the beam score log (enable_beam_score_log; needs `logprobs`)."""
         assert self.ep_world == 1 and 1 <= B <= self.max_batch
-        step = lambda: self._batched_step_kernels(B, sampled, logprobs)
+        assert not scores or (logprobs is not None and self.beam_scores is not None and self.beam_scores.shape[0] >= B)
+        step = lambda: self._batched_step_kernels(B, sampled, logprobs, scores)
         if not use_graph:
             step()
             return
         key = (B, sampled, "logprobs", logprobs) if logprobs is not None else (B, sampled)
+        if scores:
+            key += ("scores",)
         self._replay(self._bgraphs, key, step)   # one graph per batch size (continuous batching changes B)
 
     def _replay(self, graphs: dict, key, step):

@@ -13,9 +13,10 @@ from typing import List, Optional, Sequence
 import torch
 
 from .. import ops
+from ..beam import BeamSearch, check_beam_args, pack_outputs
 from ..config import VitaConfig, IMAGE_TOKEN_INDEX, AUDIO_TOKEN_INDEX
 from .internvit import InternViTVisionTower, VisionProjector
-from ..sampling import check_logprobs, from_hf
+from ..sampling import MAX_LOGPROBS, check_logprobs, from_hf
 from .mixtral import MixtralDecoder
 from .whale import AudioEncoder
 
@@ -106,6 +107,8 @@ class GenerateOutput:
     sequences: torch.Tensor
     scores: Optional[tuple] = None
     logprobs: Optional[tuple] = None      # generate(logprobs=N): one sampling.TokenLogprobs per generated token
+    sequences_scores: Optional[torch.Tensor] = None   # beam search: [R] fp32 length-penalised hypothesis scores
+    beam_indices: Optional[torch.Tensor] = None       # beam search: [R, n] running beam of each token (-1: padding)
 
 
 class CapturedEncoders:
@@ -413,7 +416,8 @@ class VITAMixtralForCausalLM:
     def generate(self, input_ids, images=None, audios=None, do_sample=False, temperature=None, top_p=None,
                  num_beams=1, output_scores=False, return_dict_in_generate=True, max_new_tokens=16, use_cache=True,
                  stopping_criteria=None, eos_token_id: Optional[int] = None, use_graph: bool = True, sync_every: int = 16,
-                 top_k=None, seed: Optional[int] = None, logprobs: Optional[int] = None, **kw):
+                 top_k=None, seed: Optional[int] = None, logprobs: Optional[int] = None, length_penalty: float = 1.0,
+                 early_stopping=False, num_return_sequences: int = 1, **kw):
         """Greedy or sampled decode with the call signature of video_audio_demo.py:257-270.  `sequences` (on
         `input_ids.device`) echoes the prompt ids, placeholders included, followed by the new tokens
         (video_audio_demo.py:272-276).
@@ -428,9 +432,17 @@ class VITAMixtralForCausalLM:
 
         The decode step replays as one CUDA graph whether or not `output_scores` is set: with scores the step appends
         its logits row to a device-resident log, and `scores` are views of that log (valid until the next call).
-        Tokens are read back every `sync_every` steps; stopping criteria see each new token exactly once."""
+        Tokens are read back every `sync_every` steps; stopping criteria see each new token exactly once.
+
+        `num_beams` > 1 (at most 10 and at most the model's `max_batch`): beam search as HF transformers runs it with
+        `length_penalty`, `early_stopping` and `num_return_sequences` (vita_b200/beam.py).  `sequences` holds the best
+        `num_return_sequences` hypotheses, padded with `eos_token_id`, with `sequences_scores` and `beam_indices`;
+        `scores` (with `output_scores`) holds one [num_beams, V] block of the running beams' log-softmax rows per step.
+        The beams share their KV pages copy-on-write and advance together through the batched decode step."""
         if num_beams != 1:
-            raise ValueError("beam search is not supported (num_beams=1)")
+            return self._beam_search(input_ids, images, audios, num_beams, num_return_sequences, length_penalty,
+                                     early_stopping, do_sample, logprobs, output_scores, return_dict_in_generate,
+                                     max_new_tokens, stopping_criteria, eos_token_id, use_graph)
         params = from_hf(do_sample, temperature, top_k, top_p, seed, **kw)
         sampled = params is not None
         n_top = check_logprobs(logprobs)
@@ -485,3 +497,103 @@ class VITAMixtralForCausalLM:
         scores = tuple(score_log[i: i + 1] for i in range(n_new)) if output_scores else None
         lps = tuple(llm.read_logprobs(0, seq_host[0, L: L + n_new].tolist(), n_top)) if want_lp else None
         return GenerateOutput(seq, scores, lps)
+
+    @torch.no_grad()
+    def _beam_search(self, input_ids, images, audios, N, R, length_penalty, early_stopping, do_sample, logprobs,
+                     output_scores, return_dict_in_generate, max_new_tokens, stopping_criteria, eos_token_id,
+                     use_graph):
+        """generate(num_beams=N > 1): prefill once into slot 0, fork it into slots 1 .. N - 1 after the first choice,
+        then one batched step over the N running beams per token.  Each step reads back every beam's top 2N
+        logprobs (one host sync), lets BeamSearch choose, and moves the beams' KV rows to their new parents."""
+        llm = self.llm
+        check_beam_args(N, R, early_stopping)
+        if do_sample:
+            raise ValueError("beam-sample decoding (num_beams > 1 with do_sample=True) is not supported")
+        if logprobs is not None:
+            raise ValueError("logprobs= is not supported with num_beams > 1")
+        if llm.ep_world > 1:
+            raise ValueError("beam search is single-GPU (the expert-parallel mode serves greedy requests)")
+        if N > llm.max_batch:
+            raise ValueError(f"num_beams={N} exceeds the model's max_batch ({llm.max_batch}): the beams run in "
+                             f"decoder slots; build the model with max_batch >= num_beams")
+        if input_ids.shape[0] != 1:
+            raise ValueError("generate() is single-sequence like the demo; use generate_batch() for more")
+        if max_new_tokens < 1:
+            raise ValueError("beam search needs max_new_tokens >= 1")
+        emb, lens = self._embeds_for(input_ids, images, audios)
+        llm.check_capacity(lens[0], max_new_tokens)
+        llm.reset()
+        try:
+            return self._run_beams(emb[0, :lens[0]].contiguous(), input_ids, N, R, length_penalty, early_stopping,
+                                   output_scores, return_dict_in_generate, max_new_tokens, stopping_criteria,
+                                   eos_token_id, use_graph)
+        finally:
+            # the decoder leaves beam search as every other path expects it: block_table rows that agree with
+            # slot_map's again (the engine's prefill writes through slot_map, the batched step reads block_table), a
+            # full pool, greedy slots
+            llm.cache.unshare()
+            for b in range(N):
+                llm.sampling.set(b, None)
+
+    def _run_beams(self, emb, input_ids, N, R, length_penalty, early_stopping, output_scores,
+                   return_dict_in_generate, max_new_tokens, stopping_criteria, eos_token_id, use_graph):
+        llm = self.llm
+        for b in range(N):
+            llm.sampling.set(b, None, MAX_LOGPROBS)
+        lp = llm.enable_logprob_log()
+        score_log = llm.enable_beam_score_log(N, max_new_tokens) if output_scores else None
+        S = emb.shape[0]
+        llm.prefill(emb, slot=0, scores=score_log[0] if output_scores else None, logprobs=MAX_LOGPROBS,
+                    log_softmax_scores=output_scores)
+        if output_scores:
+            score_log[1:N, 0].copy_(score_log[0, 0])          # step 0: HF's N identical rows of the expanded prompt
+        prompt = input_ids[0].tolist()
+        L, K = len(prompt), 2 * N
+        seq_host = torch.empty(N, L + max_new_tokens, dtype=torch.long)      # the running beams, for the criteria
+        seq_host[:, :L] = torch.tensor(prompt, dtype=torch.long)
+        ids_h = torch.empty(N, K, dtype=torch.int32, pin_memory=True)
+        lps_h = torch.empty(N, K, dtype=torch.float32, pin_memory=True)
+        search = BeamSearch(N, max_new_tokens, eos_token_id, length_penalty, early_stopping)
+        t, rows = 0, 1                 # t: tokens each running beam holds; rows: slots whose logprob row is current
+        while True:
+            ids_h[:rows].copy_(lp[2][:rows, t, :K], non_blocking=True)
+            lps_h[:rows].copy_(lp[3][:rows, t, :K], non_blocking=True)
+            torch.cuda.current_stream().synchronize()                       # the one host sync per step
+            parents = search.step(ids_h[:rows].tolist(), lps_h[:rows].numpy())
+            t += 1
+            stop = False
+            if stopping_criteria:      # every step, the last one included, as HF 4.41's beam search calls them
+                for i, beam in enumerate(search.running):
+                    seq_host[i, L:L + t] = torch.tensor(beam.tokens, dtype=torch.long)
+                scores = tuple(score_log[:N, i] for i in range(t)) if output_scores else None
+                stop = _criteria_stop(stopping_criteria, seq_host[:len(search.running), :L + t], scores)
+            if search.done:
+                break
+            if stop:
+                search.finalize()
+                break
+            if t == 1:                 # every first choice continues slot 0: fork it
+                llm.fork(0, range(1, N), S)
+            else:
+                llm.cache.reorder(parents, S + t - 1)
+            words = [0xFFFFFFFF - beam.tokens[-1] for beam in search.running]    # packed words decode_embed consumes
+            llm.best[:N].copy_(torch.tensor(words, dtype=torch.int64))
+            llm.decode_step_batched(N, use_graph=use_graph, logprobs=MAX_LOGPROBS, scores=output_scores)
+            rows = N
+        hyps = search.best(R)
+        seq, seq_scores, beam_idx = pack_outputs(hyps, prompt, eos_token_id if eos_token_id is not None else 0)
+        seq = torch.from_numpy(seq).to(input_ids.device)
+        if not return_dict_in_generate:
+            return seq
+        scores = tuple(score_log[:N, i] for i in range(t)) if output_scores else None
+        return GenerateOutput(seq, scores, None, torch.from_numpy(seq_scores), torch.from_numpy(beam_idx))
+
+
+def _criteria_stop(stopping_criteria, view: torch.Tensor, scores) -> bool:
+    """HF 4.41's StoppingCriteriaList over the running beams: a row is done when any criterion says so (a criterion
+    may return one bool for all rows); the search stops when every row is done.  `scores`: the score blocks so far
+    (output_scores) or None, as HF passes them."""
+    done = torch.zeros(view.shape[0], dtype=torch.bool)
+    for sc in stopping_criteria:
+        done |= torch.as_tensor(sc(view, scores), dtype=torch.bool).reshape(-1).expand(view.shape[0])
+    return bool(done.all())

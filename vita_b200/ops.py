@@ -241,12 +241,15 @@ def sample_rows(logits, temperature, top_k, top_p, seed, counter, best, scores: 
 
 
 def sample_logprobs(logits, temperature, top_k, top_p, seed, counter, best, logprob, rank, top_ids, top_logprobs,
-                    n_top: int, target: Optional[torch.Tensor] = None, scores: Optional[torch.Tensor] = None):
+                    n_top: int, target: Optional[torch.Tensor] = None, scores: Optional[torch.Tensor] = None,
+                    log_softmax_scores: bool = False):
     """`sample_rows` plus log-probabilities over the processed row (contract: vita_b200/sampling.py).
     `target` (i32 [B], optional): rows with target[b] in [0, V) score that token and draw nothing (best[b] gets the
     greedy word); the other rows score the token they choose.  Outputs: logprob f32 / rank i32 of shape [B] (row b) or
     [B, rows] (row counter[b] of request b, a device-resident log); top_ids i32 / top_logprobs f32 of that shape plus
-    a last dimension >= n_top (0 <= n_top <= 20): the n_top largest logits, lowest index first on ties."""
+    a last dimension >= n_top (0 <= n_top <= 20): the n_top largest logits, lowest index first on ties.
+    `log_softmax_scores`: the score rows receive bf16(logprob) of every token (HF beam search's scores) instead of the
+    processed row."""
     _chk(logits, BF16, "logits", contiguous=False); _chk(best, torch.int64, "best")
     _chk(temperature, torch.float32, "temperature"); _chk(top_p, torch.float32, "top_p")
     _chk(top_k, torch.int32, "top_k"); _chk(counter, torch.int32, "counter"); _chk(seed, torch.int64, "seed")
@@ -280,10 +283,21 @@ def sample_logprobs(logits, temperature, top_k, top_p, seed, counter, best, logp
         if scores.shape[0] < B or scores.shape[2] != V:
             raise _lib.VitaB200Error("sample_logprobs: scores must be [B, rows, V]")
         rows = scores.shape[1]
-    _lib.call("vita_sample_rows_logprobs", _p(logits), logits.stride(0), B, V, _p(temperature), _p(top_k), _p(top_p),
+    entry = "vita_sample_rows_logsoftmax" if log_softmax_scores else "vita_sample_rows_logprobs"
+    _lib.call(entry, _p(logits), logits.stride(0), B, V, _p(temperature), _p(top_k), _p(top_p),
               _p(seed), _p(counter), _p(target), _p(best), _p(scores), V, rows, _p(logprob), _p(rank),
               _p(top_ids) if n_top > 0 else None, _p(top_logprobs) if n_top > 0 else None, int(n_top), top_ld,
               out_rows, _stream())
+
+
+def kv_copy_pages(layer_base: torch.Tensor, pairs: torch.Tensor, n_pages: int, page_bytes: int):
+    """Copy page src over page dst for every (src, dst) row of pairs (i32 [n, 2]) in every cache whose base address
+    is in layer_base (i64 [n_bases]: the K and V cache of each layer, n_pages pages of page_bytes each).  One launch."""
+    _chk(layer_base, torch.int64, "layer_base"); _chk(pairs, torch.int32, "pairs")
+    if pairs.dim() != 2 or pairs.shape[1] != 2:
+        raise _lib.VitaB200Error("kv_copy_pages: pairs must be [n, 2]")
+    _lib.call("vita_kv_copy_pages", _p(layer_base), layer_base.numel(), _p(pairs), pairs.shape[0], int(n_pages),
+              int(page_bytes), _stream())
 
 
 # ------------------------------------------------------------------------------------------------ MoE (prefill)
