@@ -123,6 +123,8 @@ int vita_attention_prefill_paged(const void* q, int64_t q_token_stride, const vo
  * splits of a kv head are merged all-to-all through tagged 64-bit words when splits is 4, 8 or 16 and the grid is
  * resident at once, otherwise by the last CTA to take a ticket ("attn_tagged"). */
 int64_t vita_decode_attention_workspace_bytes(int64_t B, int64_t n_kv_heads, int64_t splits);
+/* the merge vita_decode_attention takes for (B, n_kv_heads, splits) under the current options: 1 tagged, 0 ticket */
+int vita_decode_attention_merge(int64_t B, int64_t n_kv_heads, int64_t splits);
 int vita_decode_attention(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_table,
                           const int32_t* cur_pos, void* out, void* workspace, int64_t B, int64_t n_q_heads,
                           int64_t n_kv_heads, int64_t head_dim, int64_t page_size, int64_t max_pages, int64_t splits,

@@ -33,6 +33,7 @@ SIGNATURES = {
     "vita_attention_prefill_paged": (c_int, [P, I64, P, P, I64, P, I64, P, P, P, I64, P, I64, I64, I64, I64, I64, I64,
                                              c_float, P]),
     "vita_decode_attention_workspace_bytes": (I64, [I64, I64, I64]),
+    "vita_decode_attention_merge": (c_int, [I64, I64, I64]),
     "vita_decode_attention": (c_int, [P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, c_float, I64, P]),
     "vita_decode_slots": (c_int, [P, P, P, I64, I64, I64, P]),
     "vita_argmax_rows": (c_int, [P, P, I64, I64, P]),

@@ -423,12 +423,34 @@ decode_attn_kernel(const DecodeAttnParams p, const ChainArgsDev chain VITA_TRACE
 
 using namespace vita;
 
+// The merge a launch of (B, n_kv_heads, splits) takes.  The all-to-all protocol needs the split count to divide the
+// 4 x 128 outputs into <= 128-wide slices ... and every CTA of a kv head polls its peers, so all of them have to be
+// resident at once: keep that to grids that fit the machine (two 128-thread CTAs per SM), larger batches take the ticket
+// variant (real occupancy of the tagged variant, not an estimate: every CTA of the grid polls its peers).
+static bool decode_attn_tagged(int64_t B, int64_t n_kv_heads, int64_t splits) {
+    static int resident_per_sm = -1;
+    if (resident_per_sm < 0) {
+        int n = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, decode_attn_kernel<true>, 128, 0) != cudaSuccess || n < 1) {
+            (void)cudaGetLastError();
+            n = 1;
+        }
+        resident_per_sm = n > 2 ? 2 : n;   // a chain neighbour may share the SM under programmatic launch
+    }
+    return option("attn_tagged") && (splits == 4 || splits == 8 || splits == 16) &&
+           splits * n_kv_heads * B <= static_cast<long long>(resident_per_sm) * (num_sms() > 0 ? num_sms() : 132);
+}
+
 extern "C" int64_t vita_decode_attention_workspace_bytes(int64_t B, int64_t n_kv_heads, int64_t splits) {
     // 8-byte words {value, tag} for the split partials; the ticket variant uses the front of the same buffer as plain
     // floats.  Invariant kept by both variants: the workspace is all-zero between launches (tags cleared by their
     // readers, floats zeroed by the merging CTA, tickets reset), so calls may change B / splits / variant freely.
     const int64_t n = B * n_kv_heads * splits * DEC_GROUP;
     return n * DEC_D * 8 + B * n_kv_heads * splits * splits * DEC_GROUP * 2 * 8 + ((B * n_kv_heads * 4 + 255) / 256) * 256 + 256;
+}
+
+extern "C" int vita_decode_attention_merge(int64_t B, int64_t n_kv_heads, int64_t splits) {
+    return decode_attn_tagged(B, n_kv_heads, splits) ? 1 : 0;
 }
 
 extern "C" int vita_decode_attention(const void* q, const void* k_cache, const void* v_cache,
@@ -454,21 +476,7 @@ extern "C" int vita_decode_attention(const void* q, const void* k_cache, const v
     p.scale_log2 = scale * 1.4426950408889634f;
     p.early = option("attn_early");
     dim3 grid((unsigned)splits, (unsigned)n_kv_heads, (unsigned)B);
-    // the all-to-all protocol needs the split count to divide the 4 x 128 outputs into <= 128-wide slices
-    // ... and every CTA of a kv head polls its peers, so all of them have to be resident at once: keep that to grids
-    // that fit the machine (two 128-thread CTAs per SM), larger batches take the ticket variant
-    // (real occupancy of the tagged variant, not an estimate: every CTA of the grid polls its peers)
-    static int resident_per_sm = -1;
-    if (resident_per_sm < 0) {
-        int n = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, decode_attn_kernel<true>, 128, 0) != cudaSuccess || n < 1) {
-            (void)cudaGetLastError();
-            n = 1;
-        }
-        resident_per_sm = n > 2 ? 2 : n;   // a chain neighbour may share the SM under programmatic launch
-    }
-    const bool tagged = option("attn_tagged") && (splits == 4 || splits == 8 || splits == 16) &&
-                        splits * n_kv_heads * B <= static_cast<long long>(resident_per_sm) * (num_sms() > 0 ? num_sms() : 132);
+    const bool tagged = decode_attn_tagged(B, n_kv_heads, splits);
     {
         static int carveout = -1;
         const int want = option("smem_carveout_max") ? cudaSharedmemCarveoutMaxShared : cudaSharedmemCarveoutDefault;

@@ -12,9 +12,12 @@
 
 namespace vita {
 
-// (logit, ~index) as one ordered 64-bit key: atomicMax / max picks the largest logit, the lowest index on ties
+// (logit, ~index) as one ordered 64-bit key: atomicMax / max picks the largest logit, the lowest index on ties.
+// -0.0 is packed as +0.0: the two are equal logits, so the lower index wins between them too (as in torch.argmax).
+// (NaN logits are not ordered like torch.argmax does.)
 __device__ __forceinline__ unsigned long long pack_argmax(float v, int idx) {
     uint32_t u = __float_as_uint(v);
+    if (u == 0x80000000u) u = 0u;
     u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
     return (static_cast<unsigned long long>(u) << 32) | static_cast<unsigned long long>(0xFFFFFFFFu - static_cast<uint32_t>(idx));
 }

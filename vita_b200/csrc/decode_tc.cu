@@ -813,8 +813,10 @@ struct TcDownOp {
     __device__ void finalize(int, TcFinish&) const {}
 };
 
+// same key as decode.cu's pack_argmax (-0.0 packed as +0.0, so equal logits tie on the index across warps as well)
 __device__ __forceinline__ unsigned long long tc_pack_argmax(float v, int idx) {
     uint32_t u = __float_as_uint(v);
+    if (u == 0x80000000u) u = 0u;
     u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
     return (static_cast<unsigned long long>(u) << 32) |
            static_cast<unsigned long long>(0xFFFFFFFFu - static_cast<uint32_t>(idx));

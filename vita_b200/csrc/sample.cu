@@ -41,8 +41,10 @@ __device__ __forceinline__ float key_value(uint32_t k) {
     const uint32_t u = (k & 0x8000u) ? (k & 0x7FFFu) : (~k & 0xFFFFu);
     return __uint_as_float(u << 16);
 }
+// pack_argmax's key (decode.cu): -0.0 is packed as +0.0, equal values tie on the index
 __device__ __forceinline__ unsigned long long pack_score(float v, int idx) {
     uint32_t u = __float_as_uint(v);
+    if (u == 0x80000000u) u = 0u;
     u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
     return (static_cast<unsigned long long>(u) << 32) | static_cast<unsigned long long>(0xFFFFFFFFu - static_cast<uint32_t>(idx));
 }
@@ -331,7 +333,7 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
         if (tgt >= V) tgt = -1;
     }
 
-    // stage the row as ordered keys; greedy arg-max on the way (largest key, first index)
+    // stage the row as ordered keys; greedy arg-max on the way (largest key, first index; -0.0 ties with +0.0)
     const __nv_bfloat16* row = logits + static_cast<long long>(b) * ld;
     uint32_t bk = 0u;
     int bi = 0x7fffffff;
@@ -345,8 +347,9 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
                 const uint32_t lo = bf16_key(w4[e] & 0xFFFFu), hi = bf16_key(w4[e] >> 16);
                 kk[e] = lo | (hi << 16);
                 const int i = 8 * j + 2 * e;
-                if (lo > bk || (lo == bk && i < bi)) { bk = lo; bi = i; }
-                if (hi > bk || (hi == bk && i + 1 < bi)) { bk = hi; bi = i + 1; }
+                const uint32_t cl = canon_key(lo), ch = canon_key(hi);
+                if (cl > bk || (cl == bk && i < bi)) { bk = cl; bi = i; }
+                if (ch > bk || (ch == bk && i + 1 < bi)) { bk = ch; bi = i + 1; }
             }
             reinterpret_cast<uint4*>(keys)[j] = make_uint4(kk[0], kk[1], kk[2], kk[3]);
         }
@@ -355,7 +358,8 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
         for (int i = tid; i < V; i += kSampleThreads) {
             const uint32_t kk = bf16_key(r16[i]);
             keys[i] = static_cast<uint16_t>(kk);
-            if (kk > bk || (kk == bk && i < bi)) { bk = kk; bi = i; }
+            const uint32_t ck = canon_key(kk);
+            if (ck > bk || (ck == bk && i < bi)) { bk = ck; bi = i; }
         }
     }
     const unsigned long long arg = block_max_u64(bi == 0x7fffffff ? 0ull : pack_score(key_value(bk), bi), red);
@@ -371,7 +375,10 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
         if constexpr (!LOGPROBS) return;
     }
     const uint32_t ord = static_cast<uint32_t>(arg >> 32);     // undo pack_score's float ordering, then re-key
-    const uint32_t max_key = bf16_key(((ord & 0x80000000u) ? (ord & 0x7FFFFFFFu) : ~ord) >> 16);
+    // max_key is the lowest staged key of the largest value: the thresholds below compare it with the raw keys, on
+    // which -0.0 (0x7FFF) sorts just below +0.0 (0x8000), and a maximum of zero has to keep both zeros
+    const uint32_t max_canon = bf16_key(((ord & 0x80000000u) ? (ord & 0x7FFFFFFFu) : ~ord) >> 16);
+    const uint32_t max_key = max_canon == 0x8000u ? 0x7FFFu : max_canon;
     if constexpr (LOGPROBS) {
         if (greedy) {                                    // the processed row is the logits: x = l, every token kept
             const int idx = tgt >= 0 ? tgt : static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(arg & 0xFFFFFFFFull));

@@ -191,6 +191,11 @@ def decode_attention_workspace(B: int, n_kv: int, splits: int, device) -> torch.
     return torch.zeros(n, dtype=torch.uint8, device=device)
 
 
+def decode_attention_merge(B: int, n_kv: int, splits: int) -> str:
+    """The split merge decode_attention takes for this shape under the current options: "tagged" or "ticket"."""
+    return "tagged" if _lib.load().vita_decode_attention_merge(B, n_kv, splits) else "ticket"
+
+
 def decode_attention(q, k_cache, v_cache, block_table, cur_pos, out, workspace, n_q, n_kv, head_dim, page_size,
                      splits, scale, q_stride: int = 0) -> torch.Tensor:
     _chk(q, BF16, "q", contiguous=False); _chk(k_cache, BF16, "k_cache"); _chk(v_cache, BF16, "v_cache")
