@@ -90,6 +90,15 @@ int vita_rope_kv_write(void* qkv, const int32_t* positions, const int32_t* slot_
 int vita_gemm_qkv_rope(const void* X, int64_t ldx, const void* W_qkv, void* qkv_out, int64_t M, int64_t K,
                        int64_t n_q_heads, int64_t n_kv_heads, int64_t head_dim, const int32_t* positions,
                        const int32_t* slot_mapping, const float* cos_sin, void* k_cache, void* v_cache, void* stream);
+/* FP8 (e4m3) KV cache, vLLM's kv_cache_dtype="fp8": caches of 1-byte elements in the same [slots, n_kv, head_dim]
+ * layout, one k_scale / v_scale per layer (> 0).  Write: c = e4m3_rn_satfinite(float(bf16(x)) / scale), x the row the
+ * bf16 entry point stores (fp32 division, round to nearest even, saturation at +-448).  Read: bf16(float(c) * scale).
+ * The *_fp8 entry points take the same arguments as their bf16 twins plus the two scales; every other output is
+ * bit-identical to the bf16 entry point's. */
+int vita_gemm_qkv_rope_fp8(const void* X, int64_t ldx, const void* W_qkv, void* qkv_out, int64_t M, int64_t K,
+                           int64_t n_q_heads, int64_t n_kv_heads, int64_t head_dim, const int32_t* positions,
+                           const int32_t* slot_mapping, const float* cos_sin, void* k_cache, void* v_cache,
+                           float k_scale, float v_scale, void* stream);
 
 /* ---- attention -------------------------------------------------------------------------------------------- */
 /* softmax(Q K^T * scale [causal] [kv_lens mask]) V, FlashAttention style.  Strides are {batch, token, head} in
@@ -117,6 +126,15 @@ int vita_attention_prefill_paged(const void* q, int64_t q_token_stride, const vo
                                  const int32_t* query_start_loc, const int32_t* ctx_lens, const int32_t* tiles,
                                  int64_t n_tiles, void* out, int64_t o_token_stride, int64_t T, int64_t n_q_heads,
                                  int64_t n_kv_heads, int64_t head_dim, int64_t page_size, float scale, void* stream);
+/* vita_attention_prefill_paged over e4m3 pages: for each (sequence, page index, scratch page) triple of work, page
+ * block_table[sequence * bt_stride + page index] of k_cache / v_cache is dequantized into page `scratch page` of
+ * k_out / v_out (bf16, same layout); rows at positions >= ctx_lens[sequence] are written as zeros.  The paged
+ * attention then runs on the scratch with a block table that points at the scratch pages, bit for bit the bf16 kernel
+ * over the dequantized pages. */
+int vita_kv_fp8_stage_pages(const void* k_cache, const void* v_cache, const int32_t* block_table, int64_t bt_stride,
+                            const int32_t* ctx_lens, const int32_t* work, int64_t n_work, void* k_out, void* v_out,
+                            int64_t n_kv_heads, int64_t head_dim, int64_t page_size, float k_scale, float v_scale,
+                            void* stream);
 /* single-query paged-KV attention for decode (vLLM paged Attention, mixtral.py:484-501).  workspace must be
  * zero-initialised once and be at least vita_decode_attention_workspace_bytes() large for the largest (B, splits) it
  * is used with; every launch hands it back all-zero, so B and splits may change from call to call.  The context
@@ -129,6 +147,13 @@ int vita_decode_attention(const void* q, const void* k_cache, const void* v_cach
                           const int32_t* cur_pos, void* out, void* workspace, int64_t B, int64_t n_q_heads,
                           int64_t n_kv_heads, int64_t head_dim, int64_t page_size, int64_t max_pages, int64_t splits,
                           float scale, int64_t q_stride /* elements between batch rows of q; 0 = dense */, void* stream);
+/* over e4m3 caches: each K / V element is read as bf16(float(c) * scale), the bf16 kernel's arithmetic unchanged (its
+ * output bits on the dequantized cache); same workspace, merges and chain protocol */
+int vita_decode_attention_fp8(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_table,
+                              const int32_t* cur_pos, void* out, void* workspace, int64_t B, int64_t n_q_heads,
+                              int64_t n_kv_heads, int64_t head_dim, int64_t page_size, int64_t max_pages,
+                              int64_t splits, float scale, int64_t q_stride, float k_scale, float v_scale,
+                              void* stream);
 
 /* ---- sparse MoE (prefill) --------------------------------------------------------------------------------- */
 /* post_attention_layernorm + MixtralTopKRouter (modeling_mixtral.py:109-116; vLLM FusedMoE renormalize=True,
@@ -313,6 +338,12 @@ int vita_decode_tc_qkv_rope(const void* h, const void* norm_w, const void* w_qkv
                             void* v_cache, void* workspace, int64_t ws_row_blocks, int64_t B, int64_t H,
                             int64_t n_q_heads, int64_t n_kv_heads, int64_t head_dim, int64_t page_size,
                             int64_t max_pages, float eps, void* stream);
+/* the same over e4m3 caches (see vita_gemm_qkv_rope_fp8) */
+int vita_decode_tc_qkv_rope_fp8(const void* h, const void* norm_w, const void* w_qkv, const float* cos_sin,
+                                const int32_t* cur_pos, const int32_t* block_table, void* q_out, void* k_cache,
+                                void* v_cache, void* workspace, int64_t ws_row_blocks, int64_t B, int64_t H,
+                                int64_t n_q_heads, int64_t n_kv_heads, int64_t head_dim, int64_t page_size,
+                                int64_t max_pages, float eps, float k_scale, float v_scale, void* stream);
 int vita_decode_tc_oproj(const void* x, const void* w, void* h, void* workspace, int64_t ws_row_blocks, int64_t B,
                          int64_t N, int64_t K, void* stream);
 /* route_word ([B] 64-bit words, or NULL) + route_tag (1 .. 2^32-1, different for neighbouring launches that share the

@@ -29,12 +29,16 @@ SIGNATURES = {
     "vita_row_copy": (c_int, [P, P, P, P, I64, I64, P]),
     "vita_rope_kv_write": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, P]),
     "vita_gemm_qkv_rope": (c_int, [P, I64, P, P, I64, I64, I64, I64, I64, P, P, P, P, P, P]),
+    "vita_gemm_qkv_rope_fp8": (c_int, [P, I64, P, P, I64, I64, I64, I64, I64, P, P, P, P, P, c_float, c_float, P]),
     "vita_attention_fwd": (c_int, [P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P, c_int, I64, c_float, P]),
     "vita_attention_prefill_paged": (c_int, [P, I64, P, P, I64, P, I64, P, P, P, I64, P, I64, I64, I64, I64, I64, I64,
                                              c_float, P]),
+    "vita_kv_fp8_stage_pages": (c_int, [P, P, P, I64, P, P, I64, P, P, I64, I64, I64, c_float, c_float, P]),
     "vita_decode_attention_workspace_bytes": (I64, [I64, I64, I64]),
     "vita_decode_attention_merge": (c_int, [I64, I64, I64]),
     "vita_decode_attention": (c_int, [P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, c_float, I64, P]),
+    "vita_decode_attention_fp8": (c_int, [P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, c_float, I64,
+                                          c_float, c_float, P]),
     "vita_decode_slots": (c_int, [P, P, P, I64, I64, I64, P]),
     "vita_argmax_rows": (c_int, [P, P, I64, I64, P]),
     "vita_sample_rows": (c_int, [P, I64, I64, I64, P, P, P, P, P, P, P, I64, I64, P]),
@@ -72,6 +76,8 @@ SIGNATURES = {
     "vita_decode_router": (c_int, [P, P, P, P, P, P, I64, I64, I64, c_float, P]),
     "vita_decode_tc_workspace_bytes": (I64, [I64, I64]),
     "vita_decode_tc_qkv_rope": (c_int, [P, P, P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, c_float, P]),
+    "vita_decode_tc_qkv_rope_fp8": (c_int, [P, P, P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64,
+                                            c_float, c_float, c_float, P]),
     "vita_decode_tc_oproj": (c_int, [P, P, P, P, I64, I64, I64, I64, P]),
     "vita_decode_tc_moe_gate_up": (c_int, [P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, c_float, P, I64, P]),
     "vita_decode_tc_moe_down": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, P, I64, P]),

@@ -12,6 +12,9 @@
 // (modeling_mixtral.py:269-292); vLLM paged Attention (web_demo/vllm_tools/vllm_file/mixtral.py:484-501).
 #include "common.h"
 #include "ptx.cuh"
+#include "kv_fp8.cuh"
+
+#include <type_traits>
 
 namespace vita {
 
@@ -34,6 +37,12 @@ struct DecodeAttnParams {
     float scale_log2;
     int early;                     // fetch cached K/V rows before the dependency wait
 };
+// e4m3 cache (kv_fp8.cuh): k_cache / v_cache hold 1-byte elements, read as bf16(float(c) * scale)
+struct DecodeAttnParamsFp8 : DecodeAttnParams {
+    float k_scale, v_scale;
+};
+template <bool KV8>
+using DecodeAttnArgs = std::conditional_t<KV8, DecodeAttnParamsFp8, DecodeAttnParams>;
 
 // ordered 16-byte load: volatile asm keeps it on its side of the dependency wait
 __device__ __forceinline__ uint4 ld_early_v4(const void* ptr) {
@@ -64,12 +73,15 @@ __device__ __forceinline__ float attn_rescale(float m_old, float m_new) {
 }
 
 // TAGGED = false: splits are combined by the last CTA to take a ticket (fence + atomic + reload).
+// KV8 = true    : the cache rows are e4m3 (16 bytes for the 16 dims of a lane where bf16 takes two 16-byte loads), each
+//                 element dequantized to its bf16 value before use: the same element-to-thread mapping and reduction
+//                 order, so the output bits are those of KV8 = false on the dequantized cache.
 // TAGGED = true : partials travel as 64-bit {value, tag} words in an all-to-all over the splits of a kv head: each CTA
 //                 owns a slice of the outputs and collects the other splits' words for it (no fence, no atomic, no
 //                 serial collector); lane groups are pre-merged with shuffles.
-template <bool TAGGED>
+template <bool TAGGED, bool KV8>
 __global__ void __launch_bounds__(128)
-decode_attn_kernel(const DecodeAttnParams p, const ChainArgsDev chain VITA_TRACE_PARAM) {
+decode_attn_kernel(const DecodeAttnArgs<KV8> p, const ChainArgsDev chain VITA_TRACE_PARAM) {
     __shared__ float s_m[16][DEC_GROUP];
     __shared__ float s_l[16][DEC_GROUP];
     __shared__ __align__(16) float s_o[TAGGED ? 4 : 16][DEC_GROUP][DEC_D];
@@ -118,10 +130,16 @@ decode_attn_kernel(const DecodeAttnParams p, const ChainArgsDev chain VITA_TRACE
     for (int j = 0; j < NPRE; ++j) {
         const int key = k_begin + j * 16 + lg;
         if (pslot[j] >= 0 && key != newest) {
+            if constexpr (KV8) {
+                const long long off = (pslot[j] * p.n_kv + kvh) * DEC_D + d0;
+                pk[j][0] = ld_early_v4(reinterpret_cast<const uint8_t*>(p.k_cache) + off); pk[j][1] = make_uint4(0, 0, 0, 0);
+                pv[j][0] = ld_early_v4(reinterpret_cast<const uint8_t*>(p.v_cache) + off); pv[j][1] = make_uint4(0, 0, 0, 0);
+            } else {
             const __nv_bfloat16* kp = p.k_cache + (pslot[j] * p.n_kv + kvh) * DEC_D + d0;
             const __nv_bfloat16* vp = p.v_cache + (pslot[j] * p.n_kv + kvh) * DEC_D + d0;
             pk[j][0] = ld_early_v4(kp); pk[j][1] = ld_early_v4(kp + 8);
             pv[j][0] = ld_early_v4(vp); pv[j][1] = ld_early_v4(vp + 8);
+            }
         } else {
             pk[j][0] = pk[j][1] = pv[j][0] = pv[j][1] = make_uint4(0, 0, 0, 0);
         }
@@ -133,10 +151,16 @@ decode_attn_kernel(const DecodeAttnParams p, const ChainArgsDev chain VITA_TRACE
     for (int j = 0; j < NPRE; ++j) {
         const int key = k_begin + j * 16 + lg;
         if (pslot[j] >= 0 && key == newest) {
+            if constexpr (KV8) {
+                const long long off = (pslot[j] * p.n_kv + kvh) * DEC_D + d0;
+                pk[j][0] = ld_early_v4(reinterpret_cast<const uint8_t*>(p.k_cache) + off);
+                pv[j][0] = ld_early_v4(reinterpret_cast<const uint8_t*>(p.v_cache) + off);
+            } else {
             const __nv_bfloat16* kp = p.k_cache + (pslot[j] * p.n_kv + kvh) * DEC_D + d0;
             const __nv_bfloat16* vp = p.v_cache + (pslot[j] * p.n_kv + kvh) * DEC_D + d0;
             pk[j][0] = ld_early_v4(kp); pk[j][1] = ld_early_v4(kp + 8);
             pv[j][0] = ld_early_v4(vp); pv[j][1] = ld_early_v4(vp + 8);
+            }
         }
     }
 
@@ -162,10 +186,18 @@ decode_attn_kernel(const DecodeAttnParams p, const ChainArgsDev chain VITA_TRACE
         const uint32_t kw[8] = {ka.x, ka.y, ka.z, ka.w, kc.x, kc.y, kc.z, kc.w};
         const uint32_t vw[8] = {va.x, va.y, va.z, va.w, vc.x, vc.y, vc.z, vc.w};
         float kf[16], vf[16];
+        if constexpr (KV8) {   // ka / va: 16 e4m3 bytes, byte i = dim d0 + i
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                kv_fp8_dequant4(kw[i], p.k_scale, kf + 4 * i);
+                kv_fp8_dequant4(vw[i], p.v_scale, vf + 4 * i);
+            }
+        } else {
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
             kf[2 * i] = bf16_lo(kw[i]); kf[2 * i + 1] = bf16_hi(kw[i]);
             vf[2 * i] = bf16_lo(vw[i]); vf[2 * i + 1] = bf16_hi(vw[i]);
+        }
         }
 #pragma unroll
         for (int h = 0; h < DEC_GROUP; ++h) {
@@ -197,6 +229,19 @@ decode_attn_kernel(const DecodeAttnParams p, const ChainArgsDev chain VITA_TRACE
     if (n_keys > NPRE * 16) {
         uint4 nk0, nk1, nv0, nv1;
         auto issue = [&](int key) {
+            if constexpr (KV8) {
+                nk1 = nv1 = make_uint4(0, 0, 0, 0);
+                if (key < k_end) {
+                    const int page = bt[key / p.page_size];
+                    const long long slot = static_cast<long long>(page) * p.page_size + key % p.page_size;
+                    const long long off = (slot * p.n_kv + kvh) * DEC_D + d0;
+                    nk0 = *reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(p.k_cache) + off);
+                    nv0 = *reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(p.v_cache) + off);
+                } else {
+                    nk0 = nv0 = make_uint4(0, 0, 0, 0);
+                }
+                return;
+            }
             if (key < k_end) {
                 const int page = bt[key / p.page_size];
                 const long long slot = static_cast<long long>(page) * p.page_size + key % p.page_size;
@@ -431,7 +476,7 @@ static bool decode_attn_tagged(int64_t B, int64_t n_kv_heads, int64_t splits) {
     static int resident_per_sm = -1;
     if (resident_per_sm < 0) {
         int n = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, decode_attn_kernel<true>, 128, 0) != cudaSuccess || n < 1) {
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, decode_attn_kernel<true, false>, 128, 0) != cudaSuccess || n < 1) {
             (void)cudaGetLastError();
             n = 1;
         }
@@ -453,17 +498,17 @@ extern "C" int vita_decode_attention_merge(int64_t B, int64_t n_kv_heads, int64_
     return decode_attn_tagged(B, n_kv_heads, splits) ? 1 : 0;
 }
 
-extern "C" int vita_decode_attention(const void* q, const void* k_cache, const void* v_cache,
-                                     const int32_t* block_table, const int32_t* cur_pos, void* out, void* workspace,
-                                     int64_t B, int64_t n_q_heads, int64_t n_kv_heads, int64_t head_dim,
-                                     int64_t page_size, int64_t max_pages, int64_t splits, float scale, int64_t q_stride,
-                                     void* stream) {
+template <bool KV8>
+static int decode_attention_launch(DecodeAttnArgs<KV8>& p, const void* q, const void* k_cache, const void* v_cache,
+                                   const int32_t* block_table, const int32_t* cur_pos, void* out, void* workspace,
+                                   int64_t B, int64_t n_q_heads, int64_t n_kv_heads, int64_t head_dim,
+                                   int64_t page_size, int64_t max_pages, int64_t splits, float scale, int64_t q_stride,
+                                   void* stream) {
     VITA_REQUIRE(head_dim == DEC_D && n_q_heads == n_kv_heads * DEC_GROUP, "decode attention: need D=128, GQA group 4");
     VITA_REQUIRE(splits >= 1 && splits <= 16 && workspace != nullptr, "1 <= splits <= 16 and a workspace are required");
     if (B == 0) return VITA_OK;
-    DecodeAttnParams p{};
     p.q = BF16C(q); p.q_stride = q_stride > 0 ? q_stride : n_q_heads * head_dim;
-    p.k_cache = BF16C(k_cache); p.v_cache = BF16C(v_cache);
+    p.k_cache = BF16C(k_cache); p.v_cache = BF16C(v_cache);   // e4m3 bytes when KV8 (addressed per byte)
     p.block_table = block_table; p.cur_pos = cur_pos; p.out = static_cast<__nv_bfloat16*>(out);
     const int64_t n = B * n_kv_heads * splits * DEC_GROUP;
     // tickets first (must be zero-initialised once by the caller; the kernel resets them)
@@ -481,8 +526,8 @@ extern "C" int vita_decode_attention(const void* q, const void* k_cache, const v
         static int carveout = -1;
         const int want = option("smem_carveout_max") ? cudaSharedmemCarveoutMaxShared : cudaSharedmemCarveoutDefault;
         if (carveout != want) {
-            (void)cudaFuncSetAttribute(decode_attn_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, want);
-            (void)cudaFuncSetAttribute(decode_attn_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, want);
+            (void)cudaFuncSetAttribute(decode_attn_kernel<true, KV8>, cudaFuncAttributePreferredSharedMemoryCarveout, want);
+            (void)cudaFuncSetAttribute(decode_attn_kernel<false, KV8>, cudaFuncAttributePreferredSharedMemoryCarveout, want);
             carveout = want;
         }
     }
@@ -492,8 +537,30 @@ extern "C" int vita_decode_attention(const void* q, const void* k_cache, const v
         chain = ChainArgsDev{c.serial, c.wait_cnt, c.done_cnt, c.wait_arrivals};
     }
     cudaError_t e = tagged
-        ? launch_chain(decode_attn_kernel<true>, grid, dim3(128), 0, static_cast<cudaStream_t>(stream), p, chain VITA_TRACE_ARG)
-        : launch_chain(decode_attn_kernel<false>, grid, dim3(128), 0, static_cast<cudaStream_t>(stream), p, chain VITA_TRACE_ARG);
+        ? launch_chain(decode_attn_kernel<true, KV8>, grid, dim3(128), 0, static_cast<cudaStream_t>(stream), p, chain VITA_TRACE_ARG)
+        : launch_chain(decode_attn_kernel<false, KV8>, grid, dim3(128), 0, static_cast<cudaStream_t>(stream), p, chain VITA_TRACE_ARG);
     if (e != cudaSuccess) return check_cuda(e, "decode_attn_kernel");
     return check_launch("decode_attn_kernel");
+}
+
+extern "C" int vita_decode_attention(const void* q, const void* k_cache, const void* v_cache,
+                                     const int32_t* block_table, const int32_t* cur_pos, void* out, void* workspace,
+                                     int64_t B, int64_t n_q_heads, int64_t n_kv_heads, int64_t head_dim,
+                                     int64_t page_size, int64_t max_pages, int64_t splits, float scale, int64_t q_stride,
+                                     void* stream) {
+    DecodeAttnParams p{};
+    return decode_attention_launch<false>(p, q, k_cache, v_cache, block_table, cur_pos, out, workspace, B, n_q_heads,
+                                          n_kv_heads, head_dim, page_size, max_pages, splits, scale, q_stride, stream);
+}
+
+extern "C" int vita_decode_attention_fp8(const void* q, const void* k_cache, const void* v_cache,
+                                         const int32_t* block_table, const int32_t* cur_pos, void* out, void* workspace,
+                                         int64_t B, int64_t n_q_heads, int64_t n_kv_heads, int64_t head_dim,
+                                         int64_t page_size, int64_t max_pages, int64_t splits, float scale,
+                                         int64_t q_stride, float k_scale, float v_scale, void* stream) {
+    VITA_REQUIRE(kv_fp8_scales_ok(k_scale, v_scale), "k_scale / v_scale must be finite and positive");
+    DecodeAttnParamsFp8 p{};
+    p.k_scale = k_scale; p.v_scale = v_scale;
+    return decode_attention_launch<true>(p, q, k_cache, v_cache, block_table, cur_pos, out, workspace, B, n_q_heads,
+                                         n_kv_heads, head_dim, page_size, max_pages, splits, scale, q_stride, stream);
 }

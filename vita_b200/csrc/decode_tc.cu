@@ -22,6 +22,7 @@
 #include "common.h"
 #include "ptx.cuh"
 #include "wgmma.cuh"
+#include "kv_fp8.cuh"
 
 namespace vita {
 
@@ -605,8 +606,9 @@ struct TcQkvOp {
         }
         tc_load_x_rmsnorm(h + static_cast<long long>(b) * K, norm_w, sm.xs, K, eps, sm.scratch);
     }
-    __device__ void finish(int b, int rb, int row, const float (&v)[1], TcFinish&, const TcSmem& sm) const {
-        // projections are rounded to bf16 before RoPE, as the GEMM path (and the reference) does
+    // the output row of head block rb: projections are rounded to bf16 before RoPE, as the GEMM path (and the
+    // reference) does; q and k heads are rotated
+    __device__ __forceinline__ float rope_row(int rb, int row, const float (&v)[1], const TcSmem& sm) const {
         const float x = __bfloat162float(__float2bfloat16(v[0]));
         float o = x;
         if (rb < n_q + n_kv) {   // rotate-half RoPE: partner row is row ^ 64 of the same head
@@ -618,6 +620,10 @@ struct TcQkvOp {
             o = (row < 64) ? x * c - partner * s : x * c + partner * s;
             epi_barrier();
         }
+        return o;
+    }
+    __device__ void finish(int b, int rb, int row, const float (&v)[1], TcFinish&, const TcSmem& sm) const {
+        const float o = rope_row(rb, row, v, sm);
         if (rb < n_q) {
             q_out[(static_cast<long long>(b) * n_q + rb) * 128 + row] = __float2bfloat16(o);
         } else {
@@ -628,6 +634,26 @@ struct TcQkvOp {
         }
     }
     __device__ void finalize(int, TcFinish&) const {}
+};
+
+// the same over e4m3 caches (kv_fp8.cuh): k_cache / v_cache hold bytes, each row stored as
+// e4m3_rn_satfinite(bf16(o) / scale), q unchanged
+struct TcQkvFp8Op : TcQkvOp {
+    float k_scale, v_scale;
+
+    __device__ void finish(int b, int rb, int row, const float (&v)[1], TcFinish&, const TcSmem& sm) const {
+        const float o = rope_row(rb, row, v, sm);
+        if (rb < n_q) {
+            q_out[(static_cast<long long>(b) * n_q + rb) * 128 + row] = __float2bfloat16(o);
+        } else {
+            const long long slot = sm.misc[0];
+            const bool is_k = rb < n_q + n_kv;
+            const int kvh = is_k ? rb - n_q : rb - n_q - n_kv;
+            const float ob = __bfloat162float(__float2bfloat16(o));   // the bf16 row the bf16 cache would hold
+            (reinterpret_cast<uint8_t*>(is_k ? k_cache : v_cache) + (slot * n_kv + kvh) * 128)[row] =
+                static_cast<uint8_t>(kv_fp8_quant2(ob, 0.0f, is_k ? k_scale : v_scale) & 0xffu);
+        }
+    }
 };
 
 struct TcOProjOp {
@@ -958,6 +984,28 @@ extern "C" int vita_decode_tc_qkv_rope(const void* h, const void* norm_w, const 
                (int)n_kv_heads, (int)page_size, (int)max_pages, eps};
     return launch_tc(op, w_qkv, n_rb * 128ll, (int)H, n_rb, (int)H, (int)B, split_ws(workspace, B, ws_row_blocks),
                      static_cast<cudaStream_t>(stream), "decode_tc_qkv_rope");
+}
+
+extern "C" int vita_decode_tc_qkv_rope_fp8(const void* h, const void* norm_w, const void* w_qkv, const float* cos_sin,
+                                           const int32_t* cur_pos, const int32_t* block_table, void* q_out,
+                                           void* k_cache, void* v_cache, void* workspace, int64_t ws_row_blocks,
+                                           int64_t B, int64_t H, int64_t n_q_heads, int64_t n_kv_heads,
+                                           int64_t head_dim, int64_t page_size, int64_t max_pages, float eps,
+                                           float k_scale, float v_scale, void* stream) {
+    VITA_REQUIRE(head_dim == 128 && tc_shape_ok(H), "head_dim must be 128 and H a multiple of 64");
+    VITA_REQUIRE(kv_fp8_scales_ok(k_scale, v_scale), "k_scale / v_scale must be finite and positive");
+    const int n_rb = static_cast<int>(n_q_heads + 2 * n_kv_heads);
+    VITA_REQUIRE(workspace && n_rb <= ws_row_blocks, "workspace too small");
+    if (B == 0) return VITA_OK;
+    TcQkvFp8Op op{};
+    static_cast<TcQkvOp&>(op) = TcQkvOp{BF16C(h), BF16C(norm_w), cos_sin, cur_pos, block_table,
+                                        static_cast<__nv_bfloat16*>(q_out), static_cast<__nv_bfloat16*>(k_cache),
+                                        static_cast<__nv_bfloat16*>(v_cache), (int)H, (int)n_q_heads, (int)n_kv_heads,
+                                        (int)page_size, (int)max_pages, eps};
+    op.k_scale = k_scale;
+    op.v_scale = v_scale;
+    return launch_tc(op, w_qkv, n_rb * 128ll, (int)H, n_rb, (int)H, (int)B, split_ws(workspace, B, ws_row_blocks),
+                     static_cast<cudaStream_t>(stream), "decode_tc_qkv_rope_fp8");
 }
 
 extern "C" int vita_decode_tc_oproj(const void* x, const void* w, void* h, void* workspace, int64_t ws_row_blocks,

@@ -18,6 +18,7 @@
 #include "common.h"
 #include "ptx.cuh"
 #include "wgmma.cuh"
+#include "kv_fp8.cuh"
 
 namespace vita {
 
@@ -53,6 +54,7 @@ struct GemmArgs {
     __nv_bfloat16* k_cache;
     __nv_bfloat16* v_cache;
     int n_q, n_kv;
+    float k_scale, v_scale;     // e4m3 cache (kernel template KV8): k_cache / v_cache hold bytes, kv_fp8.cuh
 };
 
 __device__ __forceinline__ void group_rows(const GemmArgs& a, int g, int& r0, int& r1) {
@@ -204,7 +206,7 @@ __device__ __forceinline__ void epi_store2(const GemmArgs& a, const EpiRow& r, c
 
 // Persistent CTA, 384 threads.  Thread 0 is the TMA producer; each consumer warpgroup owns 64 rows of the 128-row tile
 // and keeps its 64 x BLOCK_N accumulator in registers (wgmma m64nNk16, both operands from the 128B-swizzled ring).
-template <int BLOCK_N, bool SILU, int STAGES>
+template <int BLOCK_N, bool SILU, int STAGES, bool KV8 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmBs /* B in boxes of 32 rows: pieces of tail tiles */,
@@ -322,10 +324,21 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                         if (hh * 128 >= t.bn || head * 128 >= args.N) break;   // warp-uniform
                         const bool rot = head < args.n_q + args.n_kv;
                         __nv_bfloat16* cdst = nullptr;
+                        uint8_t* cdst8 = nullptr;   // KV8: e4m3 row, quantized from the bf16 values stored above
+                        float cscale = 1.0f;
+                        if constexpr (KV8) {
+                            if (slot >= 0 && head >= args.n_q) {
+                                const bool is_k = head < args.n_q + args.n_kv;
+                                const int kvh = is_k ? head - args.n_q : head - args.n_q - args.n_kv;
+                                cdst8 = reinterpret_cast<uint8_t*>(is_k ? args.k_cache : args.v_cache) + (slot * args.n_kv + kvh) * 128;
+                                cscale = is_k ? args.k_scale : args.v_scale;
+                            }
+                        } else {
                         if (slot >= 0 && head >= args.n_q) {
                             const bool is_k = head < args.n_q + args.n_kv;
                             const int kvh = is_k ? head - args.n_q : head - args.n_q - args.n_kv;
                             cdst = (is_k ? args.k_cache : args.v_cache) + (slot * args.n_kv + kvh) * 128;
+                        }
                         }
 #pragma unroll
                         for (int jb = 0; jb < 8; ++jb) {
@@ -348,9 +361,18 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                             const uint32_t o1 = pack_bf16(r1[0], r1[1]), o2 = pack_bf16(r2[0], r2[1]);
                             *reinterpret_cast<uint32_t*>(row[h].crow + head * 128 + j) = o1;
                             *reinterpret_cast<uint32_t*>(row[h].crow + head * 128 + 64 + j) = o2;
+                            if constexpr (KV8) {
+                                if (cdst8 != nullptr) {
+                                    *reinterpret_cast<uint16_t*>(cdst8 + j) =
+                                        static_cast<uint16_t>(kv_fp8_quant2(bf16_lo(o1), bf16_hi(o1), cscale));
+                                    *reinterpret_cast<uint16_t*>(cdst8 + 64 + j) =
+                                        static_cast<uint16_t>(kv_fp8_quant2(bf16_lo(o2), bf16_hi(o2), cscale));
+                                }
+                            } else {
                             if (cdst != nullptr) {
                                 *reinterpret_cast<uint32_t*>(cdst + j) = o1;
                                 *reinterpret_cast<uint32_t*>(cdst + 64 + j) = o2;
+                            }
                             }
                         }
                     }
@@ -375,12 +397,12 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     }
 }
 
-template <int BLOCK_N, bool SILU, int STAGES>
+template <int BLOCK_N, bool SILU, int STAGES, bool KV8 = false>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmBs, const GemmArgs& args,
                        int max_tiles, cudaStream_t stream) {
     constexpr int smem_bytes = STAGES * (128 * 64 * 2 + BLOCK_N * 64 * 2) + 1024 + 256;
     static bool configured = false;
-    auto kern = gemm_bf16_tn_kernel<BLOCK_N, SILU, STAGES>;
+    auto kern = gemm_bf16_tn_kernel<BLOCK_N, SILU, STAGES, KV8>;
     if (!configured) {
         int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes),
                             "cudaFuncSetAttribute(gemm smem)");
@@ -398,7 +420,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
 
 // a_rows: number of valid rows in A (TMA zero-fills beyond); b: [num_groups, b_rows, K] contiguous.
 static int gemm_dispatch(const void* A, long long lda, int a_rows, const void* B, int b_rows, const GemmArgs& args,
-                         bool silu, cudaStream_t stream) {
+                         bool silu, cudaStream_t stream, bool kv8 = false) {
     VITA_REQUIRE(args.K > 0 && args.N > 0 && args.M >= 0, "bad shape");
     VITA_REQUIRE(args.K % 8 == 0 && lda % 8 == 0, "K and lda must be multiples of 8 (16-byte TMA strides)");
     VITA_REQUIRE(aligned16(A) && aligned16(B) && aligned16(args.C), "A, B, C must be 16-byte aligned");
@@ -437,7 +459,9 @@ static int gemm_dispatch(const void* A, long long lda, int a_rows, const void* B
     };
     int block_n;
     const char* force = getenv("VITA_B200_GEMM_BN");   // tuning aid: force the tile width (128 / 256)
-    if (force && (atoi(force) == 128 || atoi(force) == 256)) {
+    if (kv8) {
+        block_n = 256;   // the e4m3 KV append has one instantiation: two whole heads per tile
+    } else if (force && (atoi(force) == 128 || atoi(force) == 256)) {
         block_n = atoi(force);
         if (!silu && args.N < 256) block_n = 128;
     } else if (silu) {
@@ -484,6 +508,7 @@ static int gemm_dispatch(const void* A, long long lda, int a_rows, const void* B
         int rc = make_tensor_map_bf16(&tmBs, B, 3, dims, strides, box, true);
         if (rc) return rc;
     }
+    if (kv8) return launch_gemm<256, false, 4, true>(tmA, tmB, tmBs, a2, max_tiles, stream);   // block_n is 256 (qkv)
     if (silu && block_n == 256) return launch_gemm<256, true, 4>(tmA, tmB, tmBs, a2, max_tiles, stream);
     if (silu) return launch_gemm<128, true, 6>(tmA, tmB, tmBs, a2, max_tiles, stream);
     if (block_n == 256) return launch_gemm<256, false, 4>(tmA, tmB, tmBs, a2, max_tiles, stream);
@@ -517,10 +542,10 @@ extern "C" int vita_gemm_bf16(const void* A, int64_t lda, const void* B, void* C
 
 // qkv projection with the RoPE + paged-KV-append epilogue (see GemmArgs): qkv_out [M, (n_q + 2 n_kv) * 128] receives the
 // rotated q and k heads and the v heads (what the prefill attention reads), k_cache / v_cache the rows of the slots.
-extern "C" int vita_gemm_qkv_rope(const void* X, int64_t ldx, const void* W_qkv, void* qkv_out, int64_t M, int64_t K,
+static int gemm_qkv_rope(const void* X, int64_t ldx, const void* W_qkv, void* qkv_out, int64_t M, int64_t K,
                                   int64_t n_q_heads, int64_t n_kv_heads, int64_t head_dim, const int32_t* positions,
                                   const int32_t* slot_mapping, const float* cos_sin, void* k_cache, void* v_cache,
-                                  void* stream) {
+                                  void* stream, bool kv8, float k_scale, float v_scale) {
     VITA_REQUIRE(head_dim == 128, "head_dim must be 128");
     VITA_REQUIRE(positions != nullptr && cos_sin != nullptr, "positions and cos_sin are required");
     VITA_REQUIRE(slot_mapping == nullptr || (k_cache != nullptr && v_cache != nullptr), "slot_mapping needs both caches");
@@ -540,7 +565,27 @@ extern "C" int vita_gemm_qkv_rope(const void* X, int64_t ldx, const void* W_qkv,
     a.v_cache = static_cast<__nv_bfloat16*>(v_cache);
     a.n_q = static_cast<int>(n_q_heads);
     a.n_kv = static_cast<int>(n_kv_heads);
-    return gemm_dispatch(X, ldx, a.M, W_qkv, a.N, a, false, static_cast<cudaStream_t>(stream));
+    a.k_scale = k_scale;
+    a.v_scale = v_scale;
+    return gemm_dispatch(X, ldx, a.M, W_qkv, a.N, a, false, static_cast<cudaStream_t>(stream), kv8);
+}
+
+extern "C" int vita_gemm_qkv_rope(const void* X, int64_t ldx, const void* W_qkv, void* qkv_out, int64_t M, int64_t K,
+                                  int64_t n_q_heads, int64_t n_kv_heads, int64_t head_dim, const int32_t* positions,
+                                  const int32_t* slot_mapping, const float* cos_sin, void* k_cache, void* v_cache,
+                                  void* stream) {
+    return gemm_qkv_rope(X, ldx, W_qkv, qkv_out, M, K, n_q_heads, n_kv_heads, head_dim, positions, slot_mapping, cos_sin,
+                         k_cache, v_cache, stream, false, 1.0f, 1.0f);
+}
+
+// the same with e4m3 caches: each K / V row is stored as e4m3_rn_satfinite(bf16 value / scale) (kv_fp8.cuh)
+extern "C" int vita_gemm_qkv_rope_fp8(const void* X, int64_t ldx, const void* W_qkv, void* qkv_out, int64_t M,
+                                      int64_t K, int64_t n_q_heads, int64_t n_kv_heads, int64_t head_dim,
+                                      const int32_t* positions, const int32_t* slot_mapping, const float* cos_sin,
+                                      void* k_cache, void* v_cache, float k_scale, float v_scale, void* stream) {
+    VITA_REQUIRE(kv_fp8_scales_ok(k_scale, v_scale), "k_scale / v_scale must be finite and positive");
+    return gemm_qkv_rope(X, ldx, W_qkv, qkv_out, M, K, n_q_heads, n_kv_heads, head_dim, positions, slot_mapping, cos_sin,
+                         k_cache, v_cache, stream, true, k_scale, v_scale);
 }
 
 extern "C" int vita_moe_gemm_gate_up_silu(const void* X_perm, const void* W_gate_up, void* Act,

@@ -185,7 +185,8 @@ def load_pretrained_model(model_path, model_base=None, model_name=None, model_ty
     if load_8bit or load_4bit:
         raise ValueError("vita_b200 runs bf16 only (bitsandbytes paths are out of scope)")
     dev = torch.device(device if device != "cuda" else "cuda:0")
-    model_kwargs = {k: kwargs[k] for k in ("max_batch", "max_seq_len", "max_new_tokens") if k in kwargs}
+    model_kwargs = {k: kwargs[k] for k in ("max_batch", "max_seq_len", "max_new_tokens", "kv_cache_dtype", "k_scale",
+                                           "v_scale") if k in kwargs}
     if str(model_path).startswith("synthetic:"):
         parts = str(model_path).split(":")
         cfg = VitaConfig.tiny() if parts[1] == "tiny" else VitaConfig.full(int(parts[2]) if len(parts) > 2 else 32)

@@ -18,6 +18,28 @@ from ..config import LLMConfig
 from ..sampling import MAX_LOGPROBS, SlotSampling, logprob_records
 
 BF16 = torch.bfloat16
+FP8 = torch.float8_e4m3fn
+
+KV_CACHE_DTYPES = {"auto": "bf16", "bf16": "bf16", "bfloat16": "bf16", "fp8": "fp8", "fp8_e4m3": "fp8"}
+
+
+def parse_kv_cache_dtype(name) -> str:
+    """vLLM's kv_cache_dtype option -> "bf16" or "fp8" (e4m3, include/vita_b200.h vita_gemm_qkv_rope_fp8).  e5m2 and
+    unknown names raise instead of being stored in a format nothing reads back."""
+    key = str(name).lower()
+    if key in KV_CACHE_DTYPES:
+        return KV_CACHE_DTYPES[key]
+    if key == "fp8_e5m2":
+        raise NotImplementedError("kv_cache_dtype 'fp8_e5m2' is not supported: the fp8 KV cache is e4m3")
+    raise ValueError(f"unknown kv_cache_dtype {name!r}; expected one of {sorted(KV_CACHE_DTYPES)}")
+
+
+def kv_scales(scale, n_layers: int, name: str) -> List[float]:
+    """A per-layer scale list from a float or a sequence of n_layers floats (vLLM's k_scale / v_scale)."""
+    vals = [float(scale)] * n_layers if isinstance(scale, (int, float)) else [float(x) for x in scale]
+    if len(vals) != n_layers or not all(v > 0.0 and v != float("inf") for v in vals):
+        raise ValueError(f"{name}: expected a positive float or {n_layers} positive floats, got {scale!r}")
+    return vals
 
 
 class PagePool:
@@ -116,15 +138,25 @@ class PagePool:
 
 
 class PagedKVCache:
-    """k/v per layer: [num_pages * page_size, n_kv_heads, head_dim] bf16; block_table [max_batch, pages_per_seq].
+    """k/v per layer: [num_pages * page_size, n_kv_heads, head_dim] bf16, or float8_e4m3fn with kv_cache_dtype "fp8"
+    (half the bytes; per-layer k_scale / v_scale, written e4m3(bf16 / scale), read bf16(e4m3 * scale));
+    block_table [max_batch, pages_per_seq].
     slot_map is derived from block_table, and the serving engine swaps the rows of both together with their slots.
     fork / reorder change block_table rows only; unshare() (and reset()) gives every slot its row from before the
     first of them back, so the two agree again."""
 
     def __init__(self, cfg: LLMConfig, max_batch: int, max_seq_len: int, device, page_size: int = 16,
-                 shuffle_pages: bool = False, storage=None):
+                 shuffle_pages: bool = False, storage=None, kv_cache_dtype: str = "auto", k_scale=1.0,
+                 v_scale=1.0):
         """`storage(layer, "k" | "v", shape) -> tensor` lets the owner place the pages (e.g. in NVLink symmetric memory
-        for the sequence-sharded expert-parallel prefill); default: ordinary device allocations."""
+        for the sequence-sharded expert-parallel prefill); default: ordinary device allocations.  `kv_cache_dtype`:
+        "auto" / "bf16" or "fp8" / "fp8_e4m3"; `k_scale` / `v_scale`: a float or one per layer (fp8 only)."""
+        self.kv_cache_dtype = parse_kv_cache_dtype(kv_cache_dtype)
+        self.dtype = FP8 if self.kv_cache_dtype == "fp8" else BF16
+        L = cfg.num_hidden_layers
+        self.k_scale, self.v_scale = kv_scales(k_scale, L, "k_scale"), kv_scales(v_scale, L, "v_scale")
+        if self.kv_cache_dtype == "bf16" and (set(self.k_scale) != {1.0} or set(self.v_scale) != {1.0}):
+            raise ValueError("k_scale / v_scale apply to the fp8 KV cache only")
         self.page_size = page_size
         self.pages_per_seq = (max_seq_len + page_size - 1) // page_size
         self.max_seq_len = self.pages_per_seq * page_size
@@ -133,7 +165,7 @@ class PagedKVCache:
         slots = n_pages * page_size
         shape = (slots, cfg.num_key_value_heads, cfg.head_dim)
         if storage is None:
-            storage = lambda layer, which, shp: torch.zeros(shp, dtype=BF16, device=device)
+            storage = lambda layer, which, shp: torch.zeros(shp, dtype=self.dtype, device=device)
         self.k = [storage(l, "k", shape) for l in range(cfg.num_hidden_layers)]
         self.v = [storage(l, "v", shape) for l in range(cfg.num_hidden_layers)]
         order = torch.randperm(n_pages, generator=torch.Generator().manual_seed(0)) if shuffle_pages \
@@ -228,23 +260,29 @@ class LayerAttention:
         return LayerAttention(whole, paged, decode, page_size)
 
     def __call__(self, qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, out: torch.Tensor,
-                 c: LLMConfig, splits: int):
+                 c: LLMConfig, splits: int, k_scale: float = 1.0, v_scale: float = 1.0):
+        """e4m3 caches (float8_e4m3fn) are read through bf16(c * scale): the paged FlashAttention over a dequantized
+        scratch of the plan's pages, the decode kernel directly.  Whole prompts attend their own bf16 rows."""
         nq, nkv, D, W = c.num_attention_heads, c.num_key_value_heads, c.head_dim, c.qkv_rows
         for r0, n in self.whole:
             q = qkv[r0:r0 + n]
             ops.attention(q, q[:, nq * D:], q[:, (nq + nkv) * D:], out[r0:r0 + n], (0, W, D), (0, W, D), (0, W, D),
                           (0, nq * D, D), 1, nq, nkv, n, n, D, D, None, True, D ** -0.5)
         if self.paged is not None:
-            ops.attention_prefill_paged(qkv, k_cache, v_cache, self.paged, out, nq, nkv, D, D ** -0.5)
+            ops.attention_prefill_paged(qkv, k_cache, v_cache, self.paged, out, nq, nkv, D, D ** -0.5, k_scale, v_scale)
         if self.decode is not None:
             r0, n, block_table, cur_pos, workspace = self.decode
             ops.decode_attention(qkv[r0:r0 + n], k_cache, v_cache, block_table, cur_pos, out[r0:r0 + n], workspace, nq,
-                                 nkv, D, self.page_size, splits, D ** -0.5, q_stride=W)
+                                 nkv, D, self.page_size, splits, D ** -0.5, q_stride=W, k_scale=k_scale,
+                                 v_scale=v_scale)
 
 
 class MixtralDecoder:
     def __init__(self, cfg: LLMConfig, weights: dict, device, max_batch: int = 1, max_seq_len: Optional[int] = None,
-                 max_new_tokens: int = 1024, page_size: int = 16, decode_splits: int = 16, shuffle_pages: bool = False):
+                 max_new_tokens: int = 1024, page_size: int = 16, decode_splits: int = 16, shuffle_pages: bool = False,
+                 kv_cache_dtype: str = "auto", k_scale=1.0, v_scale=1.0):
+        """`kv_cache_dtype`: "auto" / "bf16" (default) or "fp8" / "fp8_e4m3", an e4m3 paged KV cache at half the bytes
+        with per-layer `k_scale` / `v_scale` (a float or one per layer; vLLM's defaults are 1.0)."""
         self.cfg = cfg
         self.w = weights
         self.device = torch.device(device)
@@ -263,11 +301,14 @@ class MixtralDecoder:
         self.ep_rank, self.ep_world = weights.get("ep", (0, 1))
         self.ep_mode = "seq" if self.ep_world > 1 else None
         self.ep_p2p = None
+        if parse_kv_cache_dtype(kv_cache_dtype) == "fp8" and self.ep_world > 1:
+            raise ValueError("the fp8 KV cache is single-GPU: the expert-parallel prefill all-gathers bf16 K/V rows")
         storage = None
         if self.ep_mode == "seq":
             assert max_batch == 1 and not shuffle_pages, "sequence-sharded EP serves one sequence with in-order pages"
             storage = self._init_ep_seq(page_rounded)
-        self.cache = PagedKVCache(cfg, max_batch, max_seq_len, device, page_size, shuffle_pages, storage)
+        self.cache = PagedKVCache(cfg, max_batch, max_seq_len, device, page_size, shuffle_pages, storage,
+                                  kv_cache_dtype, k_scale, v_scale)
         self.max_new_tokens = max_new_tokens
         self.decode_splits = int(os.environ.get("VITA_B200_ATTN_SPLITS", decode_splits))
         H, I = cfg.hidden_size, cfg.intermediate_size
@@ -413,8 +454,9 @@ class MixtralDecoder:
         ops.rmsnorm(h, layers[0]["ln1"], c.rms_norm_eps, out=xn)
         for li, lw in enumerate(layers):
             # qkv projection, RoPE and the KV append in one kernel (GEMM epilogue)
-            ops.linear_qkv_rope(xn, lw["wqkv"], qkv, pos, slots, w["rope"], k_cache[li], v_cache[li], nq, nkv, D)
-            attention(qkv, k_cache[li], v_cache[li], attn, c, self.decode_splits)
+            ks, vs = self.cache.k_scale[li], self.cache.v_scale[li]
+            ops.linear_qkv_rope(xn, lw["wqkv"], qkv, pos, slots, w["rope"], k_cache[li], v_cache[li], nq, nkv, D, ks, vs)
+            attention(qkv, k_cache[li], v_cache[li], attn, c, self.decode_splits, ks, vs)
             ops.linear(attn, lw["wo"], residual=h, out=h)
             # router + permute in one kernel (slot layout), grouped GEMMs over the slots, gather-combine
             cnt = ws["cnt"][li]
@@ -582,10 +624,10 @@ class MixtralDecoder:
             for li, lw in enumerate(w["layers"]):
                 ops.decode_tc_qkv_rope(h, lw["ln1"], lw["wqkv"], w["rope"], cache.cur_pos[:B], cache.block_table[:B],
                                        self.d_q[:B], cache.k[li], cache.v[li], ws, nq, nkv, D, cache.page_size,
-                                       c.rms_norm_eps)
+                                       c.rms_norm_eps, cache.k_scale[li], cache.v_scale[li])
                 ops.decode_attention(self.d_q[:B], cache.k[li], cache.v[li], cache.block_table[:B], cache.cur_pos[:B],
                                      self.d_attn[:B], self.attn_ws, nq, nkv, D, cache.page_size, self.decode_splits,
-                                     D ** -0.5)
+                                     D ** -0.5, k_scale=cache.k_scale[li], v_scale=cache.v_scale[li])
                 ops.decode_tc_oproj(self.d_attn[:B], lw["wo"], h, ws)
                 tracing = self.route_trace is not None and not torch.cuda.is_current_stream_capturing()
                 route = None if (tracing or not self.early_route) else self.d_route[:B]

@@ -166,13 +166,17 @@ class VITAMixtralForCausalLM:
     kernel-native layout)."""
 
     def __init__(self, cfg: VitaConfig, packed: dict, device="cuda", max_batch: int = 1,
-                 max_seq_len: Optional[int] = None, max_new_tokens: int = 1024, shuffle_pages: bool = False):
+                 max_seq_len: Optional[int] = None, max_new_tokens: int = 1024, shuffle_pages: bool = False,
+                 kv_cache_dtype: str = "auto", k_scale=1.0, v_scale=1.0):
+        """`kv_cache_dtype` "fp8" / "fp8_e4m3": e4m3 paged KV cache with per-layer k_scale / v_scale (MixtralDecoder);
+        "auto" / "bf16" (default): bf16.  generate(), beam search and the serving engine run on whichever it is."""
         self.config = cfg
         self.device = torch.device(device)
         self.dtype = BF16
         self.packed = packed
         self.llm = MixtralDecoder(cfg.llm, packed["llm"], device, max_batch, max_seq_len, max_new_tokens,
-                                  shuffle_pages=shuffle_pages)
+                                  shuffle_pages=shuffle_pages, kv_cache_dtype=kv_cache_dtype, k_scale=k_scale,
+                                  v_scale=v_scale)
         self.vision_tower = InternViTVisionTower(cfg.vision, packed["vision"], device) if "vision" in packed else None
         self.mm_projector = VisionProjector(packed["projector"]) if "projector" in packed else None
         self.audio_encoder = AudioEncoder(cfg.audio, cfg.llm.hidden_size, packed["audio"], device) \

@@ -4,6 +4,7 @@ marshals pointers/sizes into one libvita_b200.so call on the current CUDA stream
 from __future__ import annotations
 
 import ctypes
+import math
 from typing import Optional
 
 import torch
@@ -12,6 +13,7 @@ from . import _lib
 
 ACT_NONE, ACT_GELU, ACT_RELU = 0, 1, 2
 BF16 = torch.bfloat16
+FP8 = torch.float8_e4m3fn      # e4m3 KV cache (include/vita_b200.h, vita_gemm_qkv_rope_fp8)
 
 
 def _stream() -> int:
@@ -29,6 +31,21 @@ def _chk(t: torch.Tensor, dtype, name: str, contiguous: bool = True):
         raise _lib.VitaB200Error(f"{name}: expected dtype {dtype}, got {t.dtype}")
     if contiguous and not t.is_contiguous():
         raise _lib.VitaB200Error(f"{name}: expected a contiguous tensor")
+
+
+def _kv_fp8(k_cache, v_cache, name: str) -> bool:
+    """True for an e4m3 cache pair, False for bf16; anything else (or a mixed pair) raises."""
+    fp8 = k_cache is not None and k_cache.dtype == FP8
+    dt = FP8 if fp8 else BF16
+    _chk(k_cache, dt, f"{name}: k_cache"); _chk(v_cache, dt, f"{name}: v_cache")
+    return fp8
+
+
+def _scales(k_scale, v_scale):
+    ks, vs = 1.0 if k_scale is None else float(k_scale), 1.0 if v_scale is None else float(v_scale)
+    if not (math.isfinite(ks) and math.isfinite(vs) and ks > 0.0 and vs > 0.0):
+        raise _lib.VitaB200Error(f"k_scale / v_scale must be finite and positive, got {ks} / {vs}")
+    return ks, vs
 
 
 def _i64arr(vals):
@@ -98,6 +115,8 @@ def rope_kv_write(qkv: torch.Tensor, positions: torch.Tensor, slot_mapping: Opti
                   cos_sin: torch.Tensor, k_cache: Optional[torch.Tensor], v_cache: Optional[torch.Tensor],
                   n_q: int, n_kv: int, head_dim: int) -> None:
     _chk(qkv, BF16, "qkv"); _chk(positions, torch.int32, "positions"); _chk(cos_sin, torch.float32, "cos_sin")
+    if k_cache is not None and k_cache.dtype == FP8:
+        raise _lib.VitaB200Error("rope_kv_write: e4m3 caches are not supported (linear_qkv_rope writes them)")
     if slot_mapping is not None:
         _chk(slot_mapping, torch.int32, "slot_mapping"); _chk(k_cache, BF16, "k_cache"); _chk(v_cache, BF16, "v_cache")
     _lib.call("vita_rope_kv_write", _p(qkv), _p(positions), _p(slot_mapping), _p(cos_sin), _p(k_cache), _p(v_cache),
@@ -106,8 +125,10 @@ def rope_kv_write(qkv: torch.Tensor, positions: torch.Tensor, slot_mapping: Opti
 
 def linear_qkv_rope(x: torch.Tensor, w_qkv: torch.Tensor, out: torch.Tensor, positions: torch.Tensor,
                     slot_mapping: Optional[torch.Tensor], cos_sin: torch.Tensor, k_cache: Optional[torch.Tensor],
-                    v_cache: Optional[torch.Tensor], n_q: int, n_kv: int, head_dim: int) -> torch.Tensor:
-    """qkv projection with RoPE + paged-KV append in the GEMM epilogue (== linear() then rope_kv_write(), one kernel)."""
+                    v_cache: Optional[torch.Tensor], n_q: int, n_kv: int, head_dim: int,
+                    k_scale: Optional[float] = None, v_scale: Optional[float] = None) -> torch.Tensor:
+    """qkv projection with RoPE + paged-KV append in the GEMM epilogue (== linear() then rope_kv_write(), one kernel).
+    e4m3 caches (float8_e4m3fn) store each row as e4m3(bf16 row / scale) with the layer's k_scale / v_scale (default 1)."""
     _chk(x, BF16, "x", contiguous=False); _chk(w_qkv, BF16, "w_qkv"); _chk(out, BF16, "out")
     _chk(positions, torch.int32, "positions"); _chk(cos_sin, torch.float32, "cos_sin")
     M, K = x.shape
@@ -115,8 +136,14 @@ def linear_qkv_rope(x: torch.Tensor, w_qkv: torch.Tensor, out: torch.Tensor, pos
         raise _lib.VitaB200Error("linear_qkv_rope: shape mismatch")
     if positions.numel() < M or (slot_mapping is not None and slot_mapping.numel() < M):
         raise _lib.VitaB200Error("linear_qkv_rope: positions / slot_mapping shorter than the row count")
+    fp8 = False
     if slot_mapping is not None:
-        _chk(slot_mapping, torch.int32, "slot_mapping"); _chk(k_cache, BF16, "k_cache"); _chk(v_cache, BF16, "v_cache")
+        _chk(slot_mapping, torch.int32, "slot_mapping"); fp8 = _kv_fp8(k_cache, v_cache, "linear_qkv_rope")
+    if fp8:
+        ks, vs = _scales(k_scale, v_scale)
+        _lib.call("vita_gemm_qkv_rope_fp8", _p(x), x.stride(0), _p(w_qkv), _p(out), M, K, n_q, n_kv, head_dim,
+                  _p(positions), _p(slot_mapping), _p(cos_sin), _p(k_cache), _p(v_cache), ks, vs, _stream())
+        return out
     _lib.call("vita_gemm_qkv_rope", _p(x), x.stride(0), _p(w_qkv), _p(out), M, K, n_q, n_kv, head_dim, _p(positions),
               _p(slot_mapping), _p(cos_sin), _p(k_cache), _p(v_cache), _stream())
     return out
@@ -165,21 +192,54 @@ class PagedPrefill:
         buf = torch.tensor([x for t in tiles for x in t[1:]] + qsl + ctx, dtype=torch.int32).to(block_table.device)
         n = 2 * len(tiles)
         self.tiles, self.qsl, self.ctx = buf[:n], buf[n:n + B + 1], buf[n + B + 1:]
+        self._seqs, self._ctx_host, self._stage = seqs, ctx, None
+
+    def fp8_stage(self, k_cache: torch.Tensor):
+        """The e4m3 path's staging of this plan, built on first use and reused by every layer: (work [n, 3] int32
+        device: (sequence, page index, scratch page) of every page a planned sequence reads, the remapped block table
+        [B, pages] pointing at the scratch pages, k / v scratch [pages * page_size, n_kv, head_dim] bf16).  The scratch
+        covers the whole context of every planned sequence (4 KiB per token for K and V together at 8 kv heads) and
+        is allocated once per plan, i.e. once per step, from torch's caching allocator."""
+        if self._stage is None:
+            ps, work = self.page_size, []
+            B = self.block_table.shape[0]
+            width = max((c + ps - 1) // ps for c in self._ctx_host) if self._ctx_host else 1
+            table = [[0] * width for _ in range(B)]
+            for i in self._seqs:
+                for pi in range((self._ctx_host[i] + ps - 1) // ps):
+                    table[i][pi] = len(work)
+                    work.append((i, pi, len(work)))
+            dev = self.block_table.device
+            n_pages = max(len(work), 1)
+            shape = (n_pages * ps,) + tuple(k_cache.shape[1:])
+            self._stage = (torch.tensor(work, dtype=torch.int32).reshape(-1, 3).to(dev),
+                           torch.tensor(table, dtype=torch.int32).to(dev),
+                           torch.empty(shape, dtype=BF16, device=dev), torch.empty(shape, dtype=BF16, device=dev))
+        return self._stage
 
 
 def attention_prefill_paged(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, plan: PagedPrefill,
-                            out: torch.Tensor, n_q: int, n_kv: int, head_dim: int, scale: float) -> torch.Tensor:
+                            out: torch.Tensor, n_q: int, n_kv: int, head_dim: int, scale: float,
+                            k_scale: Optional[float] = None, v_scale: Optional[float] = None) -> torch.Tensor:
     """Causal attention of prompt continuations over the paged cache (include/vita_b200.h).  q [T, >= n_q * head_dim]
     (rows may be strided, e.g. the packed qkv), k/v_cache [slots, n_kv, head_dim], out [T, n_q * head_dim] (rows may
     be strided); row r of sequence i attends its keys <= ctx_lens[i] - (qsl[i + 1] - qsl[i]) + r.  Rows of sequences
-    outside the plan are left as they are."""
+    outside the plan are left as they are.  e4m3 caches: the plan's pages are dequantized into a bf16 scratch first
+    (vita_kv_fp8_stage_pages, one launch) and the same kernel runs on it."""
     _chk(q, BF16, "q", contiguous=False); _chk(out, BF16, "out", contiguous=False)
-    _chk(k_cache, BF16, "k_cache"); _chk(v_cache, BF16, "v_cache")
+    fp8 = _kv_fp8(k_cache, v_cache, "attention_prefill_paged")
     if q.shape[0] != plan.T or out.shape[0] != plan.T or q.stride(1) != 1 or out.stride(1) != 1 \
             or out.shape[1] < n_q * head_dim or k_cache.shape != v_cache.shape or k_cache.dim() != 3 \
             or tuple(k_cache.shape[1:]) != (n_kv, head_dim):
         raise _lib.VitaB200Error("attention_prefill_paged: shape mismatch")
     bt = plan.block_table
+    if fp8:
+        ks, vs = _scales(k_scale, v_scale)
+        work, bt, k16, v16 = plan.fp8_stage(k_cache)
+        _lib.call("vita_kv_fp8_stage_pages", _p(k_cache), _p(v_cache), _p(plan.block_table), plan.block_table.stride(0),
+                  _p(plan.ctx), _p(work), work.shape[0], _p(k16), _p(v16), n_kv, head_dim, plan.page_size, ks, vs,
+                  _stream())
+        k_cache, v_cache = k16, v16
     _lib.call("vita_attention_prefill_paged", _p(q), q.stride(0), _p(k_cache), _p(v_cache), k_cache.shape[0], _p(bt),
               bt.stride(0), _p(plan.qsl), _p(plan.ctx), _p(plan.tiles), plan.n_tiles, _p(out), out.stride(0), plan.T,
               n_q, n_kv, head_dim, plan.page_size, float(scale), _stream())
@@ -197,11 +257,19 @@ def decode_attention_merge(B: int, n_kv: int, splits: int) -> str:
 
 
 def decode_attention(q, k_cache, v_cache, block_table, cur_pos, out, workspace, n_q, n_kv, head_dim, page_size,
-                     splits, scale, q_stride: int = 0) -> torch.Tensor:
-    _chk(q, BF16, "q", contiguous=False); _chk(k_cache, BF16, "k_cache"); _chk(v_cache, BF16, "v_cache")
+                     splits, scale, q_stride: int = 0, k_scale: Optional[float] = None,
+                     v_scale: Optional[float] = None) -> torch.Tensor:
+    """e4m3 caches are read as bf16(c * scale) with the layer's k_scale / v_scale (default 1)."""
+    _chk(q, BF16, "q", contiguous=False); fp8 = _kv_fp8(k_cache, v_cache, "decode_attention")
     _chk(out, BF16, "out")
     _chk(block_table, torch.int32, "block_table"); _chk(cur_pos, torch.int32, "cur_pos")
     B = cur_pos.shape[0]
+    if fp8:
+        ks, vs = _scales(k_scale, v_scale)
+        _lib.call("vita_decode_attention_fp8", _p(q), _p(k_cache), _p(v_cache), _p(block_table), _p(cur_pos), _p(out),
+                  _p(workspace), B, n_q, n_kv, head_dim, page_size, block_table.shape[1], splits, float(scale),
+                  q_stride, ks, vs, _stream())
+        return out
     _lib.call("vita_decode_attention", _p(q), _p(k_cache), _p(v_cache), _p(block_table), _p(cur_pos), _p(out),
               _p(workspace), B, n_q, n_kv, head_dim, page_size, block_table.shape[1], splits, float(scale), q_stride,
               _stream())
@@ -511,8 +579,15 @@ class TcWorkspace:
 
 
 def decode_tc_qkv_rope(h, norm_w, w_qkv, cos_sin, cur_pos, block_table, q_out, k_cache, v_cache, ws, n_q, n_kv,
-                       head_dim, page_size, eps):
+                       head_dim, page_size, eps, k_scale: Optional[float] = None, v_scale: Optional[float] = None):
     B, H = h.shape
+    if k_cache.dtype == FP8:
+        _kv_fp8(k_cache, v_cache, "decode_tc_qkv_rope")
+        ks, vs = _scales(k_scale, v_scale)
+        _lib.call("vita_decode_tc_qkv_rope_fp8", _p(h), _p(norm_w), _p(w_qkv), _p(cos_sin), _p(cur_pos),
+                  _p(block_table), _p(q_out), _p(k_cache), _p(v_cache), _p(ws.buf), ws.max_row_blocks, B, H, n_q, n_kv,
+                  head_dim, page_size, block_table.shape[1], float(eps), ks, vs, _stream())
+        return
     _lib.call("vita_decode_tc_qkv_rope", _p(h), _p(norm_w), _p(w_qkv), _p(cos_sin), _p(cur_pos), _p(block_table),
               _p(q_out), _p(k_cache), _p(v_cache), _p(ws.buf), ws.max_row_blocks, B, H, n_q, n_kv, head_dim, page_size,
               block_table.shape[1], float(eps), _stream())

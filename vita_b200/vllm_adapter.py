@@ -31,10 +31,23 @@ from . import ops, weights as W
 from .config import VitaConfig
 from .sampling import TokenLogprobs, check_logprobs, from_vllm, logprob_records, row_tensors
 from .model.internvit import InternViTVisionTower, VisionProjector
-from .model.mixtral import LayerAttention, MixtralDecoder
+from .model.mixtral import FP8, LayerAttention, MixtralDecoder
 from .model.whale import AudioEncoder
 
 BF16 = torch.bfloat16
+
+# vLLM's CacheConfig.cache_dtype -> the decoder's kv_cache_dtype
+CACHE_DTYPES = {"auto": "bf16", "bfloat16": "bf16", "fp8": "fp8", "fp8_e4m3": "fp8"}
+
+
+def kv_cache_dtype_of(cache_config) -> str:
+    """`cache_config.cache_dtype` ("auto" when absent) -> "bf16" or "fp8" (e4m3).  "fp8_e5m2" and every other name
+    raise NotImplementedError: the engine would otherwise allocate pages in a format the kernels misread."""
+    name = getattr(cache_config, "cache_dtype", "auto") if cache_config is not None else "auto"
+    name = "auto" if name is None else str(name)
+    if name not in CACHE_DTYPES:
+        raise NotImplementedError(f"cache_dtype {name!r} is not supported (supported: {sorted(CACHE_DTYPES)})")
+    return CACHE_DTYPES[name]
 
 
 @dataclass
@@ -77,6 +90,7 @@ class MixtralForConditionalGeneration:
         self.device = torch.device(device)
         self.image_token_index, self.audio_token_index = image_token_index, audio_token_index
         self.block_size = getattr(cache_config, "block_size", 16) if cache_config is not None else 16
+        self.kv_cache_dtype = kv_cache_dtype_of(cache_config)
         self.packed = None
         self._dec_ws = {}
         if packed is not None:
@@ -117,7 +131,8 @@ class MixtralForConditionalGeneration:
         cfg = self.config
         self.packed = packed
         # the decoder object supplies the layer loop + workspaces; its own (1-slot) KV cache is unused: the engine owns KV
-        self.llm = MixtralDecoder(cfg.llm, packed["llm"], self.device, max_batch=1, max_seq_len=64, max_new_tokens=8)
+        self.llm = MixtralDecoder(cfg.llm, packed["llm"], self.device, max_batch=1, max_seq_len=64, max_new_tokens=8,
+                                  kv_cache_dtype=self.kv_cache_dtype)
         self.vision_tower = InternViTVisionTower(cfg.vision, packed["vision"], self.device) if "vision" in packed else None
         self.vision_projector = VisionProjector(packed["projector"]) if "projector" in packed else None
         self.audio_tower = AudioEncoder(cfg.audio, cfg.llm.hidden_size, packed["audio"], self.device) \
@@ -186,10 +201,21 @@ class MixtralForConditionalGeneration:
         assert qsl[-1] == h.shape[0] and len(seq_lens) == len(qsl) - 1
         attention = LayerAttention.of_batch(qsl, seq_lens, meta.block_tables, self.block_size, self._decode_workspace)
         slots = meta.slot_mapping.to(device=self.device, dtype=torch.int32)
-        # engine-owned pages, vLLM flash layout
-        k = [kv[0].reshape(-1, c.num_key_value_heads, c.head_dim) for kv in kv_caches]
-        v = [kv[1].reshape(-1, c.num_key_value_heads, c.head_dim) for kv in kv_caches]
+        # engine-owned pages, vLLM flash layout; fp8 caches may come as uint8 views of the e4m3 bytes
+        k = [self._kv_view(kv[0]) for kv in kv_caches]
+        v = [self._kv_view(kv[1]) for kv in kv_caches]
         return self.llm.run_layers(h, positions, slots, k, v, attention, final_norm=True).clone()   # final RMSNorm(h)
+
+    def _kv_view(self, t: torch.Tensor) -> torch.Tensor:
+        c = self.config.llm
+        if self.kv_cache_dtype == "fp8":
+            if t.dtype == torch.uint8:
+                t = t.view(FP8)
+            if t.dtype != FP8:
+                raise ValueError(f"cache_dtype fp8 needs uint8 or float8_e4m3fn KV caches, got {t.dtype}")
+        elif t.dtype != BF16:
+            raise ValueError(f"cache_dtype auto / bfloat16 needs bf16 KV caches, got {t.dtype}")
+        return t.reshape(-1, c.num_key_value_heads, c.head_dim)
 
     def _decode_workspace(self, n: int) -> torch.Tensor:
         if n not in self._dec_ws:
