@@ -324,6 +324,14 @@ int vita_sample_rows_logsoftmax(const void* logits, int64_t ld, int64_t B, int64
  * sequence's cache with it. */
 int vita_kv_copy_pages(const uint64_t* layer_base, int64_t n_bases, const int32_t* pairs, int64_t n_pairs,
                        int64_t n_pages, int64_t page_bytes, void* stream);
+/* Prefix caching in the continuous batcher: one 128-bit digest of every full page of prompt rows.  rows: bf16
+ * [n_rows, H] with row stride ld (>= H, multiple of 8; 16-byte aligned base; H a multiple of 8); out: u64
+ * [n_rows / page_size, 2] (a partial last page gets no digest).  Page p's words w_0 .. w_{n-1} are its rows' first
+ * H values read as little-endian u64 (H / 4 per row), concatenated row by row; lane l of out[p] is
+ *   sum_j splitmix64_finalizer(w_j + j * 0x9E3779B97F4A7C15 + seed_l)  mod 2^64,
+ * seed_0 = 0x243F6A8885A308D3, seed_1 = 0x13198A2E03707344.  One CTA per page. */
+int vita_page_digest(const void* rows, int64_t ld, int64_t n_rows, int64_t H, int64_t page_size, uint64_t* out,
+                     void* stream);
 /* ---- greedy decode step on the tensor cores (wgmma swap-AB GEMV, stream-K) ---------------------------------
  * Every linear of the decode step as a weight-streaming GEMV on the tensor cores: the weight tile is the M operand of
  * wgmma and the activation vector as row 0 of a 16-wide N operand; (row-block, k-block) units are split evenly

@@ -47,6 +47,7 @@ SIGNATURES = {
     "vita_sample_rows_logsoftmax": (c_int, [P, I64, I64, I64, P, P, P, P, P, P, P, P, I64, I64, P, P, P, P, I64, I64,
                                             I64, P]),
     "vita_kv_copy_pages": (c_int, [P, I64, P, I64, I64, I64, P]),
+    "vita_page_digest": (c_int, [P, I64, I64, I64, I64, P, P]),
     "vita_moe_router": (c_int, [P, P, P, P, P, P, I64, I64, I64, c_float, P]),
     "vita_moe_align": (c_int, [P, P, P, P, P, P, P, I64, I64, P]),
     "vita_moe_gemm_down_ep": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, P]),

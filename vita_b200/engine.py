@@ -30,6 +30,14 @@ time is admitted this way; it sits in slot n_active, right behind the prefix, an
 request retires.  Its duplex events are decided after the final chunk, when its first token is known.  With nothing
 running the whole prompt goes in at once.
 
+Prefix caching (`DecoderEngine(prefix_cache=True)`, vLLM's enable_prefix_caching): the demos send one long prefix
+again and again (several questions about one video; every duplex turn rebuilt from the whole history).  The full
+pages of every prefilled prompt are indexed by a chain of digests of their embedding rows, so a request that repeats
+them shares those KV pages and its prefill starts at the hit length P (`prefill` returns P; `begin_prefill` returns
+(S, P) and the chunks start at P); the batcher reports it as `Request.cached_tokens`.  A negative query dropped after
+its prefill leaves its pages indexed, so the next query of the session shares its history.  Sampling and logprobs are
+unchanged by a hit: the first token comes from the same last-row logits with the request's own key at counter 0.
+
 `ContinuousBatcher` only talks to an `engine` object (prefill / step / swap / read_tokens / reset_slot / first_token,
 begin_prefill / prefill_rows for chunked admission, and read_logprobs only for requests that ask for logprobs), so the
 policy is unit-tested on the CPU with a deterministic stand-in; `DecoderEngine` binds it to `VITAMixtralForCausalLM`.
@@ -41,6 +49,7 @@ from typing import Callable, Dict, List, Optional, Sequence
 
 import torch
 
+from . import ops
 from .sampling import SamplingParams, TokenLogprobs
 
 
@@ -62,6 +71,7 @@ class Request:
     finished_step: int = -1
     tokens: List[int] = field(default_factory=list)
     token_logprobs: List[TokenLogprobs] = field(default_factory=list)   # one per kept token (with `logprobs`)
+    cached_tokens: int = 0              # prompt tokens served from the prefix cache (vLLM's num_cached_tokens)
 
 
 def swap_rows(tensors: Sequence[torch.Tensor], i: int, j: int) -> None:
@@ -96,10 +106,13 @@ class ContinuousBatcher:
                 slot = len(active)
                 self.engine.reset_slot(slot)
                 if self.prefill_chunk is None:
-                    self.engine.prefill(slot, r)
+                    r.cached_tokens = self.engine.prefill(slot, r) or 0
                     self._enter(r, active, done, step)
                 else:
-                    adm = [r, self.engine.begin_prefill(slot, r), 0]
+                    # an engine with a prefix cache returns (prompt rows, rows it already holds), others the row count
+                    res = self.engine.begin_prefill(slot, r)
+                    S, r.cached_tokens = res if isinstance(res, tuple) else (res, 0)
+                    adm = [r, S, r.cached_tokens]
             if adm is not None:
                 r, S, s0 = adm
                 n = min(self.prefill_chunk, S - s0) if active else S - s0   # nobody waiting: the rest at once
@@ -186,17 +199,34 @@ class ContinuousBatcher:
 class DecoderEngine:
     """Binds the batcher to `VITAMixtralForCausalLM`: prefill into a slot, batched decode step over the slot prefix."""
 
-    def __init__(self, model, use_graph: bool = True, overrun: int = 8, lone_fast_path: bool = False):
+    def __init__(self, model, use_graph: bool = True, overrun: int = 8, lone_fast_path: bool = False,
+                 prefix_cache: bool = False):
         """`overrun`: decode steps a finished request may still take before the batcher looks at its tokens
         (its `sync_every` - 1); reserved in the KV capacity check at admission.
         `lone_fast_path`: a step with a single running request takes the bs = 1 weight-streaming GEMV chain instead of
-        the batched GEMM step (faster; the two paths round differently, so tokens are no longer batch-invariant)."""
+        the batched GEMM step (faster; the two paths round differently, so tokens are no longer batch-invariant).
+        `prefix_cache` (vLLM's enable_prefix_caching): a request whose prompt rows repeat the full pages of a prompt
+        prefilled earlier shares their KV pages and prefills only the rest (see `_admit`).  Bit-identical to the cache
+        off with the bf16 KV cache; with fp8 a hit reads the cached pages through dequantization, which, as for chunked
+        prefill, is not bit-identical to a cold fp8 prefill.  The slot tables keep the cache's layout until the next
+        `MixtralDecoder.reset()` (every `generate()`, beam search, `generate_batch()` and `forward()` runs one, and it
+        clears the index): reset before serving the same model through an engine without the cache.  Not available
+        under expert parallelism (ValueError)."""
         self.model, self.llm, self.use_graph, self.overrun = model, model.llm, use_graph, overrun
         self.lone_fast_path = lone_fast_path
-        self._adm = None                    # (prompt rows, sampled, logprobs) of the request admitted in chunks
+        if prefix_cache and self.llm.ep_world > 1:
+            raise ValueError("prefix caching is single-GPU: the expert-parallel prefill takes whole prompts")
+        self.prefix_cache = prefix_cache
+        self.prefix_stats = {"hit_pages": 0, "missed_pages": 0}    # full prompt pages shared / computed
+        self._adm = None                    # (prompt rows, sampled, logprobs, page keys, epoch) of a chunked admission
         c = self.llm.cache
         self._slot_tensors = [c.block_table, c.slot_map, c.cache_len, c.cur_pos, self.llm.best, self.llm.token_log,
                               self.llm.gen_count, *self.llm.sampling.tensors]
+
+    @property
+    def evictions(self) -> int:
+        """Indexed pages the prefix cache has handed out again since the decoder was built."""
+        return self.llm.cache.pool.evictions
 
     def reset_slot(self, slot: int) -> None:
         c = self.llm.cache
@@ -204,29 +234,69 @@ class DecoderEngine:
             t[slot:slot + 1].zero_()
         self.llm.token_log[slot].zero_()
 
-    def prefill(self, slot: int, request: Request) -> None:
+    def _admit(self, slot: int, request: Request, rows: torch.Tensor):
+        """Prefix caching: digest the prompt's full pages (ops.page_digest), chain them into keys, take the cached
+        pages of the longest run of hits and private pages for everything else the request can write
+        (PagedKVCache.admit_prefix).  Returns (P, keys): P = the hit rows, a multiple of the page size below S (the
+        last prompt row is always computed: it yields the first token); the slot holds them from now on.
+
+        Pages are shared only below the hit length and only full prompt pages are indexed, so no shared page is ever
+        written again (no copy-on-write).  The slot's previous pages are released here, when the slot is reused."""
+        from .model.mixtral import prefix_keys
+        c = self.llm.cache
+        S, ps = rows.shape[0], c.page_size
+        keys = prefix_keys(ops.page_digest(rows, ps).cpu())
+        n_pages = -(-(S + request.max_new_tokens + self.overrun) // ps)
+        P = c.admit_prefix(slot, keys, S, n_pages)
+        self.prefix_stats["hit_pages"] += P // ps
+        self.prefix_stats["missed_pages"] += len(keys) - P // ps
+        c.cache_len[slot:slot + 1] = P
+        return P, keys
+
+    def _index(self, slot: int, keys, epoch: int) -> None:
+        """The slot's prompt prefill is complete: index its full pages (unless the cache was invalidated since)."""
+        pool = self.llm.cache.pool
+        if pool.epoch == epoch:
+            pool.insert(slot, keys)
+
+    def prefill(self, slot: int, request: Request) -> int:
+        """Prefill the request's prompt into `slot`; returns the prompt rows served from the prefix cache."""
         p = request.payload
         emb, lens = self.model._embeds_for(p["input_ids"], p.get("images"), p.get("audios"))
         self._check(request, int(lens[0]))
         self.llm.sampling.set(slot, request.sampling, request.logprobs)
-        self.llm.prefill(emb[0, : lens[0]].contiguous(), slot=slot, sampled=request.sampling is not None,
+        rows = emb[0, : lens[0]].contiguous()
+        P, keys = self._admit(slot, request, rows) if self.prefix_cache else (0, None)
+        self.llm.prefill(rows[P:], slot=slot, sampled=request.sampling is not None, start=P,
                          logprobs=self.llm.sampling.log_width(slot, 1))
+        if self.prefix_cache:
+            self._index(slot, keys, self.llm.cache.pool.epoch)
+        return P
 
-    def begin_prefill(self, slot: int, request: Request) -> int:
-        """Chunked admission: run the encoders and the splice once, keep the prompt rows; returns their count."""
+    def begin_prefill(self, slot: int, request: Request):
+        """Chunked admission: run the encoders and the splice once, keep the prompt rows; returns their count, and
+        with the prefix cache (count, rows already held from the cache): the chunks start there."""
         p = request.payload
         emb, lens = self.model._embeds_for(p["input_ids"], p.get("images"), p.get("audios"))
         S = int(lens[0])
         self._check(request, S)
         self.llm.sampling.set(slot, request.sampling, request.logprobs)
-        self._adm = (emb[0, :S].contiguous(), request.sampling is not None, self.llm.sampling.log_width(slot, 1))
-        return S
+        rows = emb[0, :S].contiguous()
+        if not self.prefix_cache:
+            self._adm = (rows, request.sampling is not None, self.llm.sampling.log_width(slot, 1))
+            return S
+        P, keys = self._admit(slot, request, rows)
+        self._adm = (rows, request.sampling is not None, self.llm.sampling.log_width(slot, 1), keys,
+                     self.llm.cache.pool.epoch)
+        return S, P
 
     def prefill_rows(self, slot: int, start: int, n: int, final: bool) -> None:
         """Prompt rows [start, start + n) of the request being admitted into `slot` (which holds its first `start`)."""
-        rows, sampled, logprobs = self._adm
+        rows, sampled, logprobs = self._adm[:3]
         self.llm.prefill(rows[start:start + n], slot=slot, sampled=sampled, start=start, final=final, logprobs=logprobs)
         if final:
+            if self.prefix_cache:
+                self._index(slot, *self._adm[3:])
             self._adm = None
 
     def _check(self, request: Request, prompt_len: int) -> None:
@@ -248,6 +318,8 @@ class DecoderEngine:
     def swap(self, i: int, j: int) -> None:
         swap_rows(self._slot_tensors, i, j)
         if i != j:
+            if self.prefix_cache:                    # the host table rows follow block_table's
+                self.llm.cache.pool.swap(i, j)
             self.llm.sampling.swap(i, j)
             if self.llm.lp_log is not None:          # the logprob log rows move with their request
                 swap_rows(self.llm.lp_log, i, j)

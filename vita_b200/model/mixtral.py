@@ -7,9 +7,11 @@ web_demo/vllm_tools/vllm_file/mixtral.py:375-628).  Host code only sequences ker
 from __future__ import annotations
 
 import gc
+import hashlib
 import os
+from collections import OrderedDict
 from dataclasses import dataclass
-from typing import Callable, List, Optional, Sequence, Tuple
+from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -42,18 +44,60 @@ def kv_scales(scale, n_layers: int, name: str) -> List[float]:
     return vals
 
 
+def prefix_keys(digests) -> List[bytes]:
+    """The prefix-cache keys of a prompt's full pages from their digests (ops.page_digest, [n, 2] int64 on the
+    host): key_i = blake2b-128(key_{i-1} || digest_i), key_{-1} empty, so a page's key depends on every row before
+    it as well as its own.  Collisions of 128-bit keys are treated as negligible: the cache belongs to one engine and
+    is not a boundary between tenants."""
+    keys, k = [], b""
+    raw = digests.to("cpu", torch.int64).contiguous().numpy().tobytes()
+    for i in range(0, len(raw), 16):
+        k = hashlib.blake2b(k + raw[i:i + 16], digest_size=16).digest()
+        keys.append(k)
+    return keys
+
+
+class PrefixIndex:
+    """Host index of the prefix cache: key -> page of the full prompt pages whose KV rows are known, and its inverse.
+    Pages without references that are indexed wait in `lru` (least recently released first) to be hit again or
+    evicted."""
+
+    def __init__(self):
+        self.page: Dict[bytes, int] = {}
+        self.key: Dict[int, bytes] = {}
+        self.lru: "OrderedDict[int, None]" = OrderedDict()
+
+    def add(self, key: bytes, pg: int) -> bool:
+        if key in self.page or pg in self.key:
+            return False
+        self.page[key], self.key[pg] = pg, key
+        return True
+
+    def remove(self, pg: int):
+        del self.page[self.key.pop(pg)]
+        self.lru.pop(pg, None)
+
+
 class PagePool:
-    """Host page tables with reference counts: copy-on-write sharing of KV pages between sequences (beam search).
+    """Host page tables with reference counts: copy-on-write sharing of KV pages between sequences (beam search) and
+    prompt-prefix sharing across requests (the continuous batcher's prefix cache).
 
     table[slot][i] is the page of positions [i * page_size, (i + 1) * page_size) of the slot, -1 for none.  At
     construction and after reset() every slot owns its row of `static`, the table at rest (rebase() takes a new one).  A forked or reordered slot holds the
     pages that cover its `length` tokens: full pages are shared (they are never written again), and the page its next
     row lands in (index length // page_size) is private to it.  refs[page] counts the table entries that point to the
-    page; pages whose count drops to 0 go to `free` and are handed out again."""
+    page; pages whose count drops to 0 go to `free` and are handed out again, or, when `index` holds them, to the
+    index's LRU list of evictable pages.
+
+    Prefix caching (admit / insert / release): a slot's row becomes the shared pages of its prompt's cached prefix,
+    then private pages for everything else it can write, then -1.  reset() (every invalidation) clears the index and
+    bumps `epoch`."""
 
     def __init__(self, static: torch.Tensor, page_size: int):
         self.static = static.to("cpu", torch.int32).clone()     # never a view of a device-side table
         self.page_size = page_size
+        self.epoch = 0
+        self.evictions = 0
         self.reset()
 
     def rebase(self, static: torch.Tensor):
@@ -67,11 +111,66 @@ class PagePool:
             for pg in row:
                 self.refs[pg] += 1
         self.free: List[int] = []
+        self.index = PrefixIndex()
+        self.epoch += 1
 
     def _drop(self, pg: int):
         self.refs[pg] -= 1
         if self.refs[pg] == 0:
-            self.free.append(pg)
+            if pg in self.index.key:
+                self.index.lru[pg] = None
+            else:
+                self.free.append(pg)
+
+    def _take(self) -> int:
+        """A page nothing references: a free one, else the least recently released indexed one (evicted)."""
+        if self.free:
+            pg = self.free.pop()
+        else:
+            assert self.index.lru, "KV page pool exhausted"
+            pg = next(iter(self.index.lru))
+            self.index.remove(pg)
+            self.evictions += 1
+        self.refs[pg] += 1
+        return pg
+
+    def release(self, slot: int):
+        """Drop the references of the slot's row, last page first (its earlier pages stay in the LRU list longer:
+        a later page is useless once an earlier one of its chain is evicted)."""
+        for i in reversed(range(len(self.table[slot]))):
+            if self.table[slot][i] >= 0:
+                self._drop(self.table[slot][i])
+                self.table[slot][i] = -1
+
+    def admit(self, slot: int, keys: Sequence[bytes], n_pages: int) -> int:
+        """The released slot takes the indexed pages of the longest run of `keys` found (refcount + 1), then private
+        pages up to `n_pages` in all.  Returns the number of hit pages.  Never fails while every slot row holds at
+        most len(static row) pages: the pool has that many pages per slot, so at least n_pages - hits of them are
+        free or evictable."""
+        row = self.table[slot]
+        assert all(pg < 0 for pg in row) and n_pages <= len(row), "admission into a slot that still holds pages"
+        hits = 0
+        for key in keys[:n_pages]:
+            pg = self.index.page.get(key)
+            if pg is None:
+                break
+            self.index.lru.pop(pg, None)
+            self.refs[pg] += 1
+            row[hits] = pg
+            hits += 1
+        assert len(self.free) + len(self.index.lru) >= n_pages - hits, "prefix-cache admission cannot fail"
+        for i in range(hits, n_pages):
+            row[i] = self._take()
+        return hits
+
+    def insert(self, slot: int, keys: Sequence[bytes]):
+        """Index the slot's first len(keys) pages (its full prompt pages) under their keys; a key or page already
+        indexed keeps its entry."""
+        for key, pg in zip(keys, self.table[slot]):
+            self.index.add(key, pg)
+
+    def swap(self, i: int, j: int):
+        self.table[i], self.table[j] = self.table[j], self.table[i]
 
     def _private_write_pages(self, slots: Sequence[int], length: int) -> List[Tuple[int, int]]:
         """Make page length // page_size of every slot private: a fresh page where there is none, a copy where it is
@@ -126,15 +225,20 @@ class PagePool:
         return self._private_write_pages(range(len(parents)), length)
 
     def check(self):
-        """Invariants: each count equals the number of table entries pointing to the page, free pages are exactly
-        those with count 0."""
+        """Invariants: each count equals the number of table entries pointing to the page; the index maps keys and
+        pages one to one; pages with count 0 are exactly the free ones (not indexed) and the evictable ones
+        (indexed, in the LRU list)."""
         count = [0] * len(self.refs)
         for row in self.table:
             for pg in row:
                 if pg >= 0:
                     count[pg] += 1
         assert count == self.refs, "reference counts do not match the tables"
-        assert sorted(self.free) == [pg for pg, c in enumerate(count) if c == 0], "free list does not match"
+        ix = self.index
+        assert len(ix.page) == len(ix.key) and all(ix.key[pg] == k for k, pg in ix.page.items()), "index is not 1:1"
+        unref = [pg for pg, c in enumerate(count) if c == 0]
+        assert sorted(self.free) == [pg for pg in unref if pg not in ix.key], "free list does not match"
+        assert sorted(ix.lru) == [pg for pg in unref if pg in ix.key], "evictable list does not match"
 
 
 class PagedKVCache:
@@ -173,11 +277,9 @@ class PagedKVCache:
         table = order.view(max_batch, self.pages_per_seq).to(torch.int32)
         self.block_table = table.to(device)
         self.pool = PagePool(table, page_size)
-        self.shared = False                  # fork / reorder changed block_table since the pool's rebase
+        self.shared = False                  # fork / reorder / admit_prefix changed the tables since the pool's rebase
         self._layer_base = None
-        pos = torch.arange(self.max_seq_len)
-        self.slot_map = (table[:, pos // page_size].to(torch.int64) * page_size + (pos % page_size)[None, :]) \
-            .to(torch.int32).to(device)                                      # [max_batch, max_seq_len]
+        self.slot_map = self._slot_map_rows(table).to(device)                # [max_batch, max_seq_len]
         self.cache_len = torch.zeros(max_batch, dtype=torch.int32, device=device)
         self.cur_pos = torch.zeros(max_batch, dtype=torch.int32, device=device)
 
@@ -193,12 +295,31 @@ class PagedKVCache:
             self.pool.rebase(self.block_table.cpu())
             self.shared = True
 
+    def _slot_map_rows(self, table: torch.Tensor) -> torch.Tensor:
+        pos, ps = torch.arange(self.max_seq_len), self.page_size
+        return (table[:, pos // ps].to(torch.int64) * ps + (pos % ps)[None, :]).to(torch.int32)
+
     def unshare(self):
-        """Give every slot back the block_table row it had before the first fork / reorder, and refill the pool."""
+        """Give every slot back the block_table (and slot_map) row it had before the first fork / reorder / prefix
+        admission, and refill the pool; this also invalidates the prefix index."""
         if self.shared:
             self.pool.reset()
             self.block_table.copy_(self.pool.static)
+            self.slot_map.copy_(self._slot_map_rows(self.pool.static))
             self.shared = False
+
+    def admit_prefix(self, slot: int, keys: Sequence[bytes], prompt_len: int, n_pages: int) -> int:
+        """Prefix caching: the slot gives up its pages, takes the cached pages of the longest run of its prompt's page
+        keys and private pages up to n_pages in all (PagePool.admit); its block_table and slot_map rows are written
+        here, once.  Returns the hit length P = page_size * min(pages found, (prompt_len - 1) // page_size): the last
+        prompt row is always computed, because it yields the first token."""
+        self._share()
+        self.pool.release(slot)
+        hits = self.pool.admit(slot, keys[:(prompt_len - 1) // self.page_size], n_pages)
+        row = torch.tensor([self.pool.table[slot]], dtype=torch.int32)
+        self.block_table[slot:slot + 1].copy_(row)
+        self.slot_map[slot:slot + 1].copy_(self._slot_map_rows(row))
+        return hits * self.page_size
 
     def fork(self, src: int, dsts: Sequence[int], length: int):
         """PagePool.fork on the device tables; the partial page is copied for the dsts in one kv_copy_pages launch."""

@@ -7,6 +7,7 @@ arithmetic (`plan_splice`, pure Python, unit-tested on CPU) + three device row-c
 """
 from __future__ import annotations
 
+import weakref
 from dataclasses import dataclass
 from typing import List, Optional, Sequence
 
@@ -115,16 +116,18 @@ class CapturedEncoders:
     """Both encoders as ONE CUDA graph per input geometry: InternViT + projector on the capture stream, Whale + adapter
     on a forked stream (the two are independent until the splice), ~430 launches replayed with one call.  Inputs are
     copied into static buffers; the returned feature tensors are the graph's own outputs and are overwritten by the
-    next call with the same geometry (the splice consumes them right away)."""
+    next call with the same geometry (the splice consumes them right away).  The model owns this object and is held
+    weakly here, so dropping the last reference to a model frees its device memory at once, not at the next garbage
+    collection of the cycle."""
 
     def __init__(self, model):
-        self.m = model
+        self._model = weakref.ref(model)
         self.graphs = {}
         self.replayed_launches = 0     # kernels executed through graph replays (bench.py's gpu_launches)
 
     @torch.no_grad()
     def __call__(self, images: torch.Tensor, feats: torch.Tensor, lengths):
-        m = self.m
+        m = self._model()
         if feats.dim() == 2:
             feats = feats.unsqueeze(0)
         lengths = torch.as_tensor(lengths).reshape(-1)

@@ -373,6 +373,18 @@ def kv_copy_pages(layer_base: torch.Tensor, pairs: torch.Tensor, n_pages: int, p
               int(page_bytes), _stream())
 
 
+def page_digest(rows: torch.Tensor, page_size: int) -> torch.Tensor:
+    """128-bit digest of every full page of prompt rows (include/vita_b200.h vita_page_digest): rows bf16 [n, H]
+    (rows may be strided) -> int64 [n // page_size, 2], the bits of the two u64 lanes.  A partial last page gets none."""
+    _chk(rows, BF16, "rows", contiguous=False)
+    if rows.dim() != 2 or rows.stride(1) != 1:
+        raise _lib.VitaB200Error("page_digest: rows must be [n, H] with contiguous rows")
+    out = torch.empty(rows.shape[0] // page_size, 2, dtype=torch.int64, device=rows.device)
+    _lib.call("vita_page_digest", _p(rows), rows.stride(0), rows.shape[0], rows.shape[1], int(page_size), _p(out),
+              _stream())
+    return out
+
+
 # ------------------------------------------------------------------------------------------------ MoE (prefill)
 def moe_router(h, norm_w, gate_w, xn, topk_ids, topk_w, eps):
     _chk(h, BF16, "h"); _chk(norm_w, BF16, "norm_w"); _chk(gate_w, BF16, "gate_w"); _chk(xn, BF16, "xn")
