@@ -17,14 +17,13 @@ import math
 import pytest
 import torch
 
-from tests.util import BF16
+from tests.util import BF16, close_rows, matmul64, same_bits
 
 pytestmark = pytest.mark.gpu
 
 NQ, NKV, D = 32, 8, 128
 SCALE = D ** -0.5
 EPS = 1e-5
-GPU_REF_ELEMS = 10 ** 8     # fp64 references of larger matrices run on the GPU
 
 
 def _cpu_randn(shape, seed, scale=1.0):
@@ -41,46 +40,9 @@ def _perm(n, seed):
     return torch.randperm(n, generator=torch.Generator().manual_seed(seed))
 
 
-def _bits(t):
-    return t.view(torch.int16) if t.dtype == BF16 else t
-
-
-def _same_bits(a, b, what):
-    assert torch.equal(_bits(a), _bits(b)), f"{what}: bits differ"
-
-
-def _f64(w):
-    """w as float64 where its fp64 products are cheap: on the GPU above GPU_REF_ELEMS elements, on the CPU below"""
-    return w.double() if w.numel() > GPU_REF_ELEMS else w.cpu().double()
-
-
-def _matmul(w, x):
-    """x [n, K] . w [N, K]^T in fp64 -> CPU float64 [n, N] (w bf16 on any device)"""
-    w64 = _f64(w)
-    return (x.to(w64.device, torch.float64) @ w64.T).cpu()
-
-
 def _rmsnorm64(h, nw):
     h = h.double().cpu()
     return h * torch.rsqrt(h.pow(2).mean(-1, keepdim=True) + EPS) * nw.double().cpu()
-
-
-def _close_rows(got, want, what, labels, rel=1.6e-2):
-    """tests.util.assert_close applied to every leading index separately: got / want [..., n]"""
-    got = got.detach().float().cpu()
-    want = want.detach().double().cpu()
-    assert got.shape == want.shape, f"{what}: shape {tuple(got.shape)} vs {tuple(want.shape)}"
-    bad = ~torch.isfinite(got).all(-1)
-    if bad.any():
-        i = bad.nonzero()[0].tolist()
-        pytest.fail(f"{what}: non-finite values at {labels(i)}")
-    err = (got.double() - want).abs().amax(-1)
-    ref = want.abs().amax(-1).clamp_min(1e-6)
-    r = err / ref
-    if (r > rel).any():
-        i = list(divmod(int(r.argmax()), r.shape[-1])) if r.dim() == 2 else [int(r.argmax())]
-        pytest.fail(f"{what}: max err {float(err[tuple(i)]):.4e} vs max|ref| {float(ref[tuple(i)]):.4e} "
-                    f"(rel {float(r[tuple(i)]):.3e} > {rel}) at {labels(i)}")
 
 
 @pytest.fixture
@@ -187,7 +149,7 @@ def test_decode_attention_shapes(lib_options, splits, page, ctxs):
                              D, page, splits, SCALE, q_stride=q_stride)
         torch.cuda.synchronize()
         assert int(ws.count_nonzero()) == 0, f"workspace not all-zero after the launch (B={n})"
-        _same_bits(out[n], sentinel, f"out row {n} past the batch")
+        same_bits(out[n], sentinel, f"out row {n} past the batch")
         return out[:n].clone()
 
     label = lambda i: f"row {i[0]} (ctx {ctxs[i[0]]}), head {i[1]}" if len(i) == 2 else f"row {i}"
@@ -198,20 +160,20 @@ def test_decode_attention_shapes(lib_options, splits, page, ctxs):
         for layout, (q_arg, stride) in (("compact", (q_d, 0)), ("strided", (qkv[:, :NQ * D], W))):
             lib_options("attn_early", 1)
             o = run(q_arg, stride)
-            _same_bits(run(q_arg, stride), o, f"{path} merge, {layout} q: second launch on the same workspace")
+            same_bits(run(q_arg, stride), o, f"{path} merge, {layout} q: second launch on the same workspace")
             lib_options("attn_early", 0)
-            _same_bits(run(q_arg, stride), o, f"{path} merge, {layout} q: attn_early 0 vs 1")
+            same_bits(run(q_arg, stride), o, f"{path} merge, {layout} q: attn_early 0 vs 1")
             lib_options("attn_early", 1)
-            _close_rows(o.view(B, NQ, D), ref, f"decode attention, {path} merge, {layout} q, splits {splits}, "
+            close_rows(o.view(B, NQ, D), ref, f"decode attention, {path} merge, {layout} q, splits {splits}, "
                         f"page {page}", label)
             got[layout] = o
-        _same_bits(got["strided"], got["compact"], f"{path} merge: strided vs compact q")
+        same_bits(got["strided"], got["compact"], f"{path} merge: strided vs compact q")
         if B > 1:
             if ops.decode_attention_merge(1, NKV, splits) != path:
                 continue
             for b in range(B):
                 o1 = run(q_d[b:b + 1], 0, slice(b, b + 1))
-                _same_bits(o1[0], got["compact"][b], f"{path} merge: row {b} (ctx {ctxs[b]}) at B = 1 vs in B = {B}")
+                same_bits(o1[0], got["compact"][b], f"{path} merge: row {b} (ctx {ctxs[b]}) at B = 1 vs in B = {B}")
 
 
 # ================================================================================================ B. tensor-core GEMVs
@@ -249,7 +211,7 @@ def test_tc_qkv_rope_kv_append(geom, page):
 
     # fp64 reference: bf16(rmsnorm) . W, rounded to bf16 before RoPE (as the kernel and the GEMM path do)
     x = _rmsnorm64(h, nw).to(BF16)
-    y = _matmul(w, x).to(BF16).double()                                                 # [B, R]
+    y = matmul64(w, x).to(BF16).double()                                                 # [B, R]
     cs = table.double().view(4096, 128)
     heads = y.view(B, NQ + 2 * NKV, D)
     rot = heads.clone()
@@ -282,19 +244,19 @@ def test_tc_qkv_rope_kv_append(geom, page):
     rows = list(range(B))
     q, kc, vc = run(rows)
     label = lambda i: f"row {i[0]} (pos {positions[i[0]]}), head {i[1]}"
-    _close_rows(q.view(B, NQ, D), q_ref, f"qkv q (page {page})", label)
+    close_rows(q.view(B, NQ, D), q_ref, f"qkv q (page {page})", label)
     idx = torch.tensor(slots, device="cuda")
-    _close_rows(kc[idx], k_ref, f"qkv k cache append (page {page})", label)
-    _close_rows(vc[idx], v_ref, f"qkv v cache append (page {page})", label)
+    close_rows(kc[idx], k_ref, f"qkv k cache append (page {page})", label)
+    close_rows(vc[idx], v_ref, f"qkv v cache append (page {page})", label)
     q2, kc2, vc2 = run(rows)
     for a, b_, n in ((q, q2, "q"), (kc, kc2, "k cache"), (vc, vc2, "v cache")):
-        _same_bits(b_, a, f"qkv {n}: second launch on the same workspace")
+        same_bits(b_, a, f"qkv {n}: second launch on the same workspace")
     if geom == "full":
         for b in rows:
             q1, kc1, vc1 = run([b])
-            _same_bits(q1[0], q[b], f"qkv q row {b} at B = 1 vs in B = {B}")
-            _same_bits(kc1[slots[b]], kc[slots[b]], f"qkv k slot of row {b} at B = 1 vs in B = {B}")
-            _same_bits(vc1[slots[b]], vc[slots[b]], f"qkv v slot of row {b} at B = 1 vs in B = {B}")
+            same_bits(q1[0], q[b], f"qkv q row {b} at B = 1 vs in B = {B}")
+            same_bits(kc1[slots[b]], kc[slots[b]], f"qkv k slot of row {b} at B = 1 vs in B = {B}")
+            same_bits(vc1[slots[b]], vc[slots[b]], f"qkv v slot of row {b} at B = 1 vs in B = {B}")
 
 
 def _forced_moe_inputs(H, pairs, n_blocks, seed):
@@ -352,21 +314,21 @@ def _moe_check(h, nw, gw, w13, w2, pairs, resid, what, runs_at_b1=False):
     down_ref = resid.double().clone()
     for e in sorted({e for p in pairs for e in p}):          # only the experts in use, each matrix converted once
         uses = [(b, k) for b, p in enumerate(pairs) for k in range(2) if p[k] == e]
-        gu = _matmul(w13[e], torch.stack([x[b] for b, _ in uses]))
-        dn = _matmul(w2[e], torch.stack([act[b, k] for b, k in uses]))   # the down projection of the kernel's act
+        gu = matmul64(w13[e], torch.stack([x[b] for b, _ in uses]))
+        dn = matmul64(w2[e], torch.stack([act[b, k] for b, k in uses]))   # the down projection of the kernel's act
         for n, (b, k) in enumerate(uses):
             act_ref[b, k] = torch.nn.functional.silu(gu[n, :I]) * gu[n, I:]
             down_ref[b] += top_v[b, k] * dn[n]
-    _close_rows(act, act_ref, f"{what}: gate|up activations",
+    close_rows(act, act_ref, f"{what}: gate|up activations",
                 lambda i: f"token {i[0]} (experts {pairs[i[0]]}), slot {i[1]}")
-    _close_rows(out, down_ref, f"{what}: down + residual", lambda i: f"token {i[0]} (experts {pairs[i[0]]})")
+    close_rows(out, down_ref, f"{what}: down + residual", lambda i: f"token {i[0]} (experts {pairs[i[0]]})")
     again = run(rows)
     for a, b_, n in zip((act, ids, tw, out), again, ("act", "ids", "weights", "out")):
-        _same_bits(b_, a, f"{what}: {n}, second launch on the same workspace")
+        same_bits(b_, a, f"{what}: {n}, second launch on the same workspace")
     if runs_at_b1:
         for b in rows:
             for a, b_, n in zip((act, ids, tw, out), run([b]), ("act", "ids", "weights", "out")):
-                _same_bits(b_[0], a[b], f"{what}: {n} of token {b} at B = 1 vs in B = {B}")
+                same_bits(b_[0], a[b], f"{what}: {n} of token {b} at B = 1 vs in B = {B}")
 
 
 ALL_PAIRS = [(i, j) for i in range(8) for j in range(8) if i != j]
@@ -409,7 +371,7 @@ def test_tc_oproj_stream_k_extremes(N, K):
     h = _cpu_randn((B, N), N + K + 1)
     w = _gpu_randn((N, K), N + K + 2, 1.0 / math.sqrt(K))
     ws = _ws(B, (N + 127) // 128)
-    ref = h.double() + _matmul(w, x)
+    ref = h.double() + matmul64(w, x)
 
     def run(rows):
         out = h[rows].cuda()
@@ -419,10 +381,10 @@ def test_tc_oproj_stream_k_extremes(N, K):
 
     rows = list(range(B))
     out = run(rows)
-    _close_rows(out, ref, f"oproj N={N} K={K}", lambda i: f"row {i[0]}")
-    _same_bits(run(rows), out, f"oproj N={N} K={K}: second launch on the same workspace")
+    close_rows(out, ref, f"oproj N={N} K={K}", lambda i: f"row {i[0]}")
+    same_bits(run(rows), out, f"oproj N={N} K={K}: second launch on the same workspace")
     for b in rows:
-        _same_bits(run([b])[0], out[b], f"oproj N={N} K={K}: row {b} at B = 1 vs in B = {B}")
+        same_bits(run([b])[0], out[b], f"oproj N={N} K={K}: row {b} at B = 1 vs in B = {B}")
 
 
 # ================================================================================================ C. arg-max contract
@@ -500,15 +462,15 @@ def test_lm_head_argmax_ties(H, V):
     w = w_full[:V]
     logits, best = _lm_head(h, nw, w)
     x = _rmsnorm64(h, nw).to(BF16)
-    ref = _matmul(w, x)
-    _close_rows(logits, ref, f"lm head logits V={V}", lambda i: f"row {i[0]}")
+    ref = matmul64(w, x)
+    close_rows(logits, ref, f"lm head logits V={V}", lambda i: f"row {i[0]}")
     for b, (i, j) in enumerate(pairs):
         assert logits[b, i].item() == logits[b, j].item() == logits[b].float().max().item(), \
             f"row {b}: the tie at ({i}, {j}) is not the maximum"
     _check_argmax(logits, best, f"lm head ties V={V}")
     assert _unpack(best) == [i for i, _ in pairs]
     l1, b1 = _lm_head(h[:1], nw, w)
-    _same_bits(l1[0], logits[0], f"lm head logits row 0 at B = 1 vs in B = {B}")
+    same_bits(l1[0], logits[0], f"lm head logits row 0 at B = 1 vs in B = {B}")
     assert torch.equal(b1[0], best[0]), f"lm head: arg-max word of row 0 at B = 1 vs in B = {B}"
 
 

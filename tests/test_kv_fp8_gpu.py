@@ -12,9 +12,10 @@ import math
 import pytest
 import torch
 
-from tests.test_decode_shapes_gpu import (ATTN_CASES, D, EPS, NKV, NQ, SCALE, _attn_ref, _close_rows, _cpu_randn,
-                                          _gpu_randn, _paged_cache, _perm, _same_bits)
+from tests.test_decode_shapes_gpu import (ATTN_CASES, D, EPS, NKV, NQ, SCALE, _attn_ref, _cpu_randn, _gpu_randn,
+                                          _paged_cache, _perm)
 from tests.test_kv_fp8 import BF16, FP8, dequantize, qdq, quantize
+from tests.util import close_rows, same_bits
 from vita_b200 import weights as W
 from vita_b200.config import VitaConfig
 
@@ -79,7 +80,7 @@ def test_gemm_qkv_rope_store(M, ks, vs):
     ops.linear_qkv_rope(x, w, out, pos, sm, table, kc, vc, NQ, NKV, D)
     ops.linear_qkv_rope(x, w, out8, pos, sm, table, kc8, vc8, NQ, NKV, D, ks, vs)
     torch.cuda.synchronize()
-    _same_bits(out8, out, "qkv rows")
+    same_bits(out8, out, "qkv rows")
     assert _check_store(kc, vc, kc8, vc8, slots, ks, vs, f"qkv GEMM M={M}"), "no saturating row was stored"
 
 
@@ -113,7 +114,7 @@ def test_tc_qkv_rope_store(B, ks, vs):
     ops.decode_tc_qkv_rope(h, nw, w, *args, q8, kc8, vc8, ws, NQ, NKV, D, page, EPS, ks, vs)
     torch.cuda.synchronize()
     assert int(ws.buf.count_nonzero()) == 0
-    _same_bits(q8, q, "q rows")
+    same_bits(q8, q, "q rows")
     assert _check_store(kc, vc, kc8, vc8, slots, ks, vs, f"qkv GEMV B={B}"), "no saturating row was stored"
 
 
@@ -166,8 +167,8 @@ def test_decode_attention_fp8(lib_options, splits, page, ctxs):
             lib_options("attn_early", early)
             want = run(kd, vd)
             got = run(k8, v8, k_scale=ks, v_scale=vs)
-            _same_bits(got, want, f"{path} merge, attn_early {early}: fp8 vs bf16 on dequant(cache)")
-        _close_rows(got.view(B, NQ, D), ref, f"fp8 decode attention, {path} merge", label)
+            same_bits(got, want, f"{path} merge, attn_early {early}: fp8 vs bf16 on dequant(cache)")
+        close_rows(got.view(B, NQ, D), ref, f"fp8 decode attention, {path} merge", label)
 
 
 # ------------------------------------------------------------------------------------------------ paged prefill
@@ -221,9 +222,9 @@ def test_paged_prefill_fp8(P, page):
         ops.attention_prefill_paged(q, kg.cuda(), vg.cuda(), plan, got, NQ, NKV, D, SCALE, ks, vs)
         torch.cuda.synchronize()
         assert torch.isfinite(got.float()).all()
-        _same_bits(got, want, f"P={P}: fp8 paged prefill vs bf16 on dequant(pages)")
+        same_bits(got, want, f"P={P}: fp8 paged prefill vs bf16 on dequant(pages)")
         results.append(got)
-    _same_bits(results[1], results[0], f"P={P}: bytes past the contexts changed the output")
+    same_bits(results[1], results[0], f"P={P}: bytes past the contexts changed the output")
 
 
 # ------------------------------------------------------------------------------------------------ model
