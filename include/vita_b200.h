@@ -315,6 +315,18 @@ int vita_sample_rows_logsoftmax(const void* logits, int64_t ld, int64_t B, int64
                                 const int32_t* counter, const int32_t* target, uint64_t* best, void* scores,
                                 int64_t score_ld, int64_t score_rows, float* logprob, int32_t* rank, int32_t* top_ids,
                                 float* top_logprobs, int64_t n_top, int64_t top_ld, int64_t out_rows, void* stream);
+/* The three sampler entry points above with a per-row stream index: streams (may be NULL: 0 everywhere) [B] i32, the
+ * third Philox counter word of row b's draw, counter (r >> 2, counter[b], streams[b], 0).  The sequences of one
+ * request share its key and draw from streams 0 .. N-1 (parallel sampling); stream 0 is bit for bit the entry points
+ * above.  With logprob and rank both NULL this is vita_sample_rows (target must be NULL and log_softmax 0);
+ * otherwise vita_sample_rows_logprobs, or vita_sample_rows_logsoftmax when log_softmax != 0.  Read after the
+ * programmatic-dependency wait like every other input. */
+int vita_sample_rows_streams(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
+                             const int32_t* top_k, const float* top_p, const uint64_t* seed, const int32_t* counter,
+                             const int32_t* streams, const int32_t* target, uint64_t* best, void* scores,
+                             int64_t score_ld, int64_t score_rows, float* logprob, int32_t* rank, int32_t* top_ids,
+                             float* top_logprobs, int64_t n_top, int64_t top_ld, int64_t out_rows,
+                             int64_t log_softmax, void* stream);
 /* Copy-on-write of the paged KV cache (vLLM's copy_blocks): for every (src, dst) page pair of pairs [n_pairs, 2] i32
  * (device) and every cache of layer_base [n_bases] (device pointers: the K and the V cache of each layer, each
  * n_pages pages of page_bytes bytes, 16-byte aligned), copy page src over page dst.  One launch, 16-byte vector

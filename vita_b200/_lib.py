@@ -46,6 +46,8 @@ SIGNATURES = {
                                           I64, P]),
     "vita_sample_rows_logsoftmax": (c_int, [P, I64, I64, I64, P, P, P, P, P, P, P, P, I64, I64, P, P, P, P, I64, I64,
                                             I64, P]),
+    "vita_sample_rows_streams": (c_int, [P, I64, I64, I64, P, P, P, P, P, P, P, P, P, I64, I64, P, P, P, P, I64, I64,
+                                         I64, I64, P]),
     "vita_kv_copy_pages": (c_int, [P, I64, P, I64, I64, I64, P]),
     "vita_page_digest": (c_int, [P, I64, I64, I64, I64, P, P]),
     "vita_moe_router": (c_int, [P, P, P, P, P, P, I64, I64, I64, c_float, P]),

@@ -7,8 +7,11 @@
 //   top-p (p < 1): over the softmax of the top-k survivors keep r iff the mass of the survivors whose logit is strictly
 //                  greater than l_r is < p (tied values are kept or dropped together); the largest logit always stays
 //   draw: argmax_r over the kept set of x_r + g_r (lowest index on ties), g_r = -log(-log(u_r)),
-//         u_r = ((w >> 8) + 0.5) * 2^-24, w = word (r & 3) of Philox4x32-10(counter (r >> 2, n, 0, 0),
-//         key (seed lo, seed hi)), n = counter[b]
+//         u_r = ((w >> 8) + 0.5) * 2^-24, w = word (r & 3) of Philox4x32-10(counter (r >> 2, n, s, 0),
+//         key (seed lo, seed hi)), n = counter[b], s = streams[b] (0 without a stream array)
+// Streams: the sequences of one request (parallel sampling: generate(num_return_sequences=N), Request.n / best_of)
+// share its key and draw from streams s = 0 .. N-1, so they are independent and reproducible from one seed, and
+// sequence 0 draws what a single-sequence request with the same key draws.
 // Logits are bf16 and the temperature is monotone, so both thresholds are found by radix selection over the 16-bit
 // ordered keys of the logits (two 256-bin passes each): top-k over counts, top-p over fixed-point masses
 // exp(x_r - x_max) * 2^40 summed as u64 (integer sums: the result does not depend on the order of the additions).
@@ -306,7 +309,7 @@ __global__ void __launch_bounds__(kSampleThreads, 1)
 sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, const float* __restrict__ temperature,
                    const int* __restrict__ top_k, const float* __restrict__ top_p,
                    const unsigned long long* __restrict__ seed, const int* __restrict__ counter,
-                   unsigned long long* __restrict__ best, __nv_bfloat16* __restrict__ scores, long long score_ld,
+                   const int* __restrict__ streams, unsigned long long* __restrict__ best, __nv_bfloat16* __restrict__ scores, long long score_ld,
                    int score_rows, int vec, LogprobArgs lp) {
     extern __shared__ __align__(16) uint8_t smem_s[];
     unsigned long long* whist = reinterpret_cast<unsigned long long*>(smem_s);
@@ -320,13 +323,15 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
     const int tid = threadIdx.x;
     // Nothing is read before the wait: the logits come from the preceding kernel, and the counter (the decoder's
     // gen_count) is written on the device earlier in the same step by a kernel that triggers its dependents before
-    // that write -- only griddepcontrol.wait makes it visible, whatever the chain options.
+    // that write -- only griddepcontrol.wait makes it visible, whatever the chain options.  The parameter arrays and
+    // the streams are read after it as well.
     pdl_wait();
     const float T = temperature[b];
     const int k = top_k[b];
     const float p = top_p[b];
     const unsigned long long key = seed[b];
     const int n = counter[b];
+    const uint32_t sid = streams != nullptr ? static_cast<uint32_t>(streams[b]) : 0u;
     int tgt = -1;
     if constexpr (LOGPROBS) {
         if (lp.target != nullptr) tgt = lp.target[b];
@@ -448,7 +453,7 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
             if (srow != nullptr && i < V) srow[i] = kept[e] ? __float2bfloat16(x[e]) : __float2bfloat16(-INFINITY);
         }
         if (!need) continue;
-        const uint4 w = philox4x32_10(make_uint4(static_cast<uint32_t>(j), static_cast<uint32_t>(n), 0u, 0u), k0, k1);
+        const uint4 w = philox4x32_10(make_uint4(static_cast<uint32_t>(j), static_cast<uint32_t>(n), sid, 0u), k0, k1);
         const uint32_t ww[4] = {w.x, w.y, w.z, w.w};
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
@@ -486,8 +491,8 @@ namespace {
 template <bool LOGPROBS, bool LSM = false>
 int launch_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
                        const int32_t* top_k, const float* top_p, const uint64_t* seed, const int32_t* counter,
-                       uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows, const LogprobArgs& lp,
-                       void* stream) {
+                       const int32_t* streams, uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows,
+                       const LogprobArgs& lp, void* stream) {
     VITA_REQUIRE(V > 0 && ld >= V, "need 0 < V <= ld");
     VITA_REQUIRE(temperature && top_k && top_p && seed && counter && best, "parameter arrays are required");
     VITA_REQUIRE(scores == nullptr || (score_ld >= V && score_rows > 0), "score log: need score_ld >= V, rows > 0");
@@ -521,7 +526,7 @@ int launch_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, con
     // logits and never triggers its own dependents early, so the next step starts after its last write of `best`
     cudaError_t e = launch_chain(sample_rows_kernel<LOGPROBS, LSM>, dim3(static_cast<unsigned>(B)), dim3(kSampleThreads), smem,
                                  static_cast<cudaStream_t>(stream), BF16C(logits), (long long)ld, (int)V, temperature,
-                                 top_k, top_p, reinterpret_cast<const unsigned long long*>(seed), counter,
+                                 top_k, top_p, reinterpret_cast<const unsigned long long*>(seed), counter, streams,
                                  reinterpret_cast<unsigned long long*>(best), static_cast<__nv_bfloat16*>(scores),
                                  (long long)score_ld, (int)score_rows, vec, lp);
     if (e != cudaSuccess) return check_cuda(e, "sample_rows");
@@ -531,29 +536,51 @@ int launch_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, con
 template <bool LSM>
 int launch_logprobs(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
                     const int32_t* top_k, const float* top_p, const uint64_t* seed, const int32_t* counter,
-                    const int32_t* target, uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows,
-                    float* logprob, int32_t* rank, int32_t* top_ids, float* top_logprobs, int64_t n_top,
-                    int64_t top_ld, int64_t out_rows, void* stream) {
+                    const int32_t* streams, const int32_t* target, uint64_t* best, void* scores, int64_t score_ld,
+                    int64_t score_rows, float* logprob, int32_t* rank, int32_t* top_ids, float* top_logprobs,
+                    int64_t n_top, int64_t top_ld, int64_t out_rows, void* stream) {
     VITA_REQUIRE(logprob && rank, "logprob and rank outputs are required");
     VITA_REQUIRE(n_top >= 0 && n_top <= kMaxTopLogprobs && n_top <= V, "need 0 <= n_top <= min(20, V)");
     VITA_REQUIRE(n_top == 0 || (top_ids && top_logprobs && top_ld >= n_top), "top-N outputs: need top_ld >= n_top");
     VITA_REQUIRE(out_rows >= 0, "out_rows must be >= 0");
     const LogprobArgs lp{target, logprob, rank, top_ids, top_logprobs, (int)n_top, (int)top_ld, (int)out_rows};
-    return launch_sample_rows<true, LSM>(logits, ld, B, V, temperature, top_k, top_p, seed, counter, best, scores,
-                                         score_ld, score_rows, lp, stream);
+    return launch_sample_rows<true, LSM>(logits, ld, B, V, temperature, top_k, top_p, seed, counter, streams, best,
+                                         scores, score_ld, score_rows, lp, stream);
 }
 
 }  // namespace
 
+extern "C" int vita_sample_rows_streams(const void* logits, int64_t ld, int64_t B, int64_t V,
+                                        const float* temperature, const int32_t* top_k, const float* top_p,
+                                        const uint64_t* seed, const int32_t* counter, const int32_t* streams,
+                                        const int32_t* target, uint64_t* best, void* scores, int64_t score_ld,
+                                        int64_t score_rows, float* logprob, int32_t* rank, int32_t* top_ids,
+                                        float* top_logprobs, int64_t n_top, int64_t top_ld, int64_t out_rows,
+                                        int64_t log_softmax, void* stream) {
+    if (logprob == nullptr && rank == nullptr) {
+        VITA_REQUIRE(target == nullptr && log_softmax == 0, "target / log-softmax scores need the logprob outputs");
+        return launch_sample_rows<false>(logits, ld, B, V, temperature, top_k, top_p, seed, counter, streams, best,
+                                         scores, score_ld, score_rows, LogprobArgs{}, stream);
+    }
+    if (log_softmax)
+        return launch_logprobs<true>(logits, ld, B, V, temperature, top_k, top_p, seed, counter, streams, target, best,
+                                     scores, score_ld, score_rows, logprob, rank, top_ids, top_logprobs, n_top, top_ld,
+                                     out_rows, stream);
+    return launch_logprobs<false>(logits, ld, B, V, temperature, top_k, top_p, seed, counter, streams, target, best,
+                                  scores, score_ld, score_rows, logprob, rank, top_ids, top_logprobs, n_top, top_ld,
+                                  out_rows, stream);
+}
+
 extern "C" int vita_sample_rows(const void* logits, int64_t ld, int64_t B, int64_t V, const float* temperature,
                                 const int32_t* top_k, const float* top_p, const uint64_t* seed, const int32_t* counter,
                                 uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows, void* stream) {
-    return launch_sample_rows<false>(logits, ld, B, V, temperature, top_k, top_p, seed, counter, best, scores, score_ld,
-                                     score_rows, LogprobArgs{}, stream);
+    return vita_sample_rows_streams(logits, ld, B, V, temperature, top_k, top_p, seed, counter, nullptr, nullptr, best,
+                                    scores, score_ld, score_rows, nullptr, nullptr, nullptr, nullptr, 0, 0, 0, 0,
+                                    stream);
 }
 
-#define VITA_LOGPROBS_ARGS logits, ld, B, V, temperature, top_k, top_p, seed, counter, target, best, scores, score_ld, \
-                           score_rows, logprob, rank, top_ids, top_logprobs, n_top, top_ld, out_rows, stream
+#define VITA_LOGPROBS_ARGS logits, ld, B, V, temperature, top_k, top_p, seed, counter, nullptr, target, best, scores, \
+                           score_ld, score_rows, logprob, rank, top_ids, top_logprobs, n_top, top_ld, out_rows
 
 extern "C" int vita_sample_rows_logprobs(const void* logits, int64_t ld, int64_t B, int64_t V,
                                          const float* temperature, const int32_t* top_k, const float* top_p,
@@ -561,7 +588,8 @@ extern "C" int vita_sample_rows_logprobs(const void* logits, int64_t ld, int64_t
                                          uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows,
                                          float* logprob, int32_t* rank, int32_t* top_ids, float* top_logprobs,
                                          int64_t n_top, int64_t top_ld, int64_t out_rows, void* stream) {
-    return launch_logprobs<false>(VITA_LOGPROBS_ARGS);
+    VITA_REQUIRE(logprob && rank, "logprob and rank outputs are required");
+    return vita_sample_rows_streams(VITA_LOGPROBS_ARGS, 0, stream);
 }
 
 extern "C" int vita_sample_rows_logsoftmax(const void* logits, int64_t ld, int64_t B, int64_t V,
@@ -570,5 +598,6 @@ extern "C" int vita_sample_rows_logsoftmax(const void* logits, int64_t ld, int64
                                            uint64_t* best, void* scores, int64_t score_ld, int64_t score_rows,
                                            float* logprob, int32_t* rank, int32_t* top_ids, float* top_logprobs,
                                            int64_t n_top, int64_t top_ld, int64_t out_rows, void* stream) {
-    return launch_logprobs<true>(VITA_LOGPROBS_ARGS);
+    VITA_REQUIRE(logprob && rank, "logprob and rank outputs are required");
+    return vita_sample_rows_streams(VITA_LOGPROBS_ARGS, 1, stream);
 }

@@ -38,9 +38,17 @@ them shares those KV pages and its prefill starts at the hit length P (`prefill`
 its prefill leaves its pages indexed, so the next query of the session shares its history.  Sampling and logprobs are
 unchanged by a hit: the first token comes from the same last-row logits with the request's own key at counter 0.
 
+Parallel sampling (`Request.n` / `Request.best_of`, vLLM 0.5.5's SamplingParams): a request asks for several sampled
+answers to one prompt.  Its group of best_of (default n) sequences waits until that many slots are free (first come,
+first served: a later arrival never overtakes it), is prefilled once, whole or in chunks, and is then forked into the
+slots right behind it (`engine.fork`): the sequences share the prompt's KV pages and draw from streams 0 .. best_of - 1
+of the request's key.  Each sequence retires on its own like a request; the request completes with its last one.
+With best_of > n the n sequences with the highest cumulative logprob are kept.
+
 `ContinuousBatcher` only talks to an `engine` object (prefill / step / swap / read_tokens / reset_slot / first_token,
-begin_prefill / prefill_rows for chunked admission, and read_logprobs only for requests that ask for logprobs), so the
-policy is unit-tested on the CPU with a deterministic stand-in; `DecoderEngine` binds it to `VITAMixtralForCausalLM`.
+begin_prefill / prefill_rows for chunked admission, read_logprobs only for requests that ask for logprobs, and fork
+only for requests with best_of > 1), so the policy is unit-tested on the CPU with a deterministic stand-in;
+`DecoderEngine` binds it to `VITAMixtralForCausalLM`.
 """
 from __future__ import annotations
 
@@ -72,6 +80,65 @@ class Request:
     tokens: List[int] = field(default_factory=list)
     token_logprobs: List[TokenLogprobs] = field(default_factory=list)   # one per kept token (with `logprobs`)
     cached_tokens: int = 0              # prompt tokens served from the prefix cache (vLLM's num_cached_tokens)
+    n: int = 1                          # sequences returned (parallel sampling; sampled requests only)
+    best_of: Optional[int] = None       # sequences generated, the n with the highest cumulative logprob kept; None = n
+    sequences: List["SequenceOutput"] = field(default_factory=list)   # filled in: the n results, tokens = sequences[0]
+
+
+@dataclass
+class SequenceOutput:
+    """One returned sequence of a request: its stream index within the request, its tokens and outcome, the logprob
+    records of its tokens (when the request asks for logprobs) and their summed logprob (when it asks for logprobs or
+    best_of > n; None otherwise)."""
+    index: int
+    tokens: List[int]
+    outcome: str
+    token_logprobs: List[TokenLogprobs] = field(default_factory=list)
+    cumulative_logprob: Optional[float] = None
+
+
+def group_size(r: Request) -> int:
+    """Sequences the request runs: best_of, or n when best_of is None."""
+    return r.n if r.best_of is None else r.best_of
+
+
+def log_width(r: Request) -> Optional[int]:
+    """The top-N the request's slots record: its own `logprobs`, else 0 when best_of > n (the ranking needs each token's
+    logprob), else None."""
+    if r.logprobs is not None:
+        return r.logprobs
+    return 0 if group_size(r) > r.n else None
+
+
+def check_request(r: Request, max_batch: int) -> None:
+    """ValueError for an n / best_of the batcher cannot serve (vLLM 0.5.5's checks where they exist)."""
+    for name, v in (("n", r.n), ("best_of", r.best_of)):
+        if v is not None and (isinstance(v, bool) or not isinstance(v, int) or v < 1):
+            raise ValueError(f"request {r.rid}: {name} must be a positive int, got {v!r}")
+    k = group_size(r)
+    if k < r.n:
+        raise ValueError(f"request {r.rid}: best_of ({r.best_of}) must be >= n ({r.n})")
+    if k > 1 and r.sampling is None:
+        raise ValueError(f"request {r.rid}: greedy sampling needs n = 1 and best_of = 1 (got n={r.n}, "
+                         f"best_of={r.best_of})")
+    if k > max_batch:
+        raise ValueError(f"request {r.rid}: best_of / n = {k} exceeds max_batch = {max_batch}")
+    if k > 1 and (r.session is not None or r.negative_token_id is not None):
+        raise ValueError(f"request {r.rid}: n / best_of > 1 cannot be combined with the duplex fields "
+                         f"(session, negative_token_id)")
+
+
+class _Fork:
+    """One sequence of a request with best_of > 1 while it runs: it occupies a slot and retires like a request of its
+    own (the fields the batcher reads), then reports to its request."""
+    session = negative_token_id = None
+
+    def __init__(self, req: Request, index: int):
+        self.req, self.index = req, index
+        self.rid, self.max_new_tokens, self.eos_token_id = req.rid, req.max_new_tokens, req.eos_token_id
+        self.logprobs = log_width(req)
+        self.steps, self.tokens, self.token_logprobs = 0, [], []
+        self.outcome, self.finished_step = "", -1
 
 
 def swap_rows(tensors: Sequence[torch.Tensor], i: int, j: int) -> None:
@@ -94,6 +161,9 @@ class ContinuousBatcher:
     def run(self, requests: Sequence[Request], on_step: Optional[Callable[[int, int], None]] = None) -> Dict[int, List[int]]:
         """Runs every request to completion; returns {rid: generated tokens (cut after EOS / max_new_tokens)}.
         `on_step(step_index, n_active)` is called after each decode-step launch (latency harnesses record events)."""
+        for r in requests:
+            check_request(r, self.max_batch)
+            r.sequences = []
         pending = sorted(requests, key=lambda r: (r.arrival_step, r.rid))
         active: List[Request] = []          # active[s] lives in slot s
         done: Dict[int, List[int]] = {}
@@ -101,7 +171,9 @@ class ContinuousBatcher:
         since_sync = 0
         adm = None                          # chunked admission in progress: [request, prompt rows, rows prefilled]
         while pending or active or adm is not None:
-            while adm is None and pending and pending[0].arrival_step <= step and len(active) < self.max_batch:
+            # first come, first served: the oldest arrival waits until its whole group of slots is free
+            while adm is None and pending and pending[0].arrival_step <= step and \
+                    len(active) + group_size(pending[0]) <= self.max_batch:
                 r = pending.pop(0)
                 slot = len(active)
                 self.engine.reset_slot(slot)
@@ -143,13 +215,18 @@ class ContinuousBatcher:
         """The prompt of `r` (in slot len(active)) is prefilled: decide its duplex events, then join the decode batch."""
         slot = len(active)
         r.admitted_step, r.steps = step, 0
+        k = group_size(r)
+        if k > 1:                                            # the group's other sequences go right behind it
+            self.engine.fork(slot, k, r.max_new_tokens)
+            active.extend(_Fork(r, i) for i in range(k))
+            return
         if r.negative_token_id is not None or r.session is not None:
             first = self.engine.first_token(slot)            # the state token: known right after the prefill
             if r.negative_token_id is not None and first == r.negative_token_id:
                 # negative audio: never enters the decode batch (the slot is simply reused by the next arrival)
                 r.tokens, r.finished_step, r.outcome = [first], step, "negative"
                 self._logprobs(r, slot)
-                done[r.rid] = r.tokens
+                self._done(r, done, step)
                 return
             if r.session is not None:                        # a real query: interrupt the running answer
                 for old_slot in sorted((i for i, o in enumerate(active) if o.session == r.session), reverse=True):
@@ -157,7 +234,7 @@ class ContinuousBatcher:
                     old.tokens = self.engine.read_tokens(old_slot)[: min(old.steps, old.max_new_tokens)]
                     old.finished_step, old.outcome = step, "interrupted"
                     self._logprobs(old, old_slot)
-                    done[old.rid] = old.tokens
+                    self._done(old, done, step)
                     last = len(active) - 1
                     # the new request sits in slot len(active) (not yet appended): move it down with the rest
                     if old_slot != last:
@@ -171,6 +248,25 @@ class ContinuousBatcher:
         """The logprob records of r's kept tokens, read before its slot is reused (only for requests that ask)."""
         if r.logprobs is not None:
             r.token_logprobs = self.engine.read_logprobs(slot, r.tokens, r.logprobs)
+
+    def _done(self, r, done: Dict[int, List[int]], step: int) -> None:
+        """A request or a sequence of a group has its outcome: record it; a group completes with its last sequence."""
+        req = r.req if isinstance(r, _Fork) else r
+        k = group_size(req)
+        lp = r.token_logprobs if req.logprobs is not None else []
+        cum = sum(t.logprob for t in r.token_logprobs) if log_width(req) is not None else None
+        req.steps = max(req.steps, r.steps)
+        req.sequences.append(SequenceOutput(r.index if isinstance(r, _Fork) else 0, r.tokens, r.outcome, lp, cum))
+        if len(req.sequences) < k:
+            return
+        seqs = sorted(req.sequences, key=lambda q: q.index)
+        if k > req.n:                                    # vLLM's ordering: highest cumulative logprob first
+            seqs = sorted(seqs, key=lambda q: (-q.cumulative_logprob, q.index))[: req.n]
+        req.sequences = seqs
+        if k > 1:
+            req.tokens, req.token_logprobs = seqs[0].tokens, seqs[0].token_logprobs
+            req.outcome, req.finished_step = "finished", step
+        done[req.rid] = req.tokens
 
     def _retire(self, active: List[Request], done: Dict[int, List[int]], step: int, admitting: bool = False) -> None:
         finished = []
@@ -187,7 +283,7 @@ class ContinuousBatcher:
                 finished.append(slot)
         for slot in sorted(finished, reverse=True):     # highest slot first: the swap partner is never a finished one
             last = len(active) - 1
-            done[active[slot].rid] = active[slot].tokens
+            self._done(active[slot], done, step)
             if slot != last:
                 self.engine.swap(slot, last)
                 active[slot] = active[last]
@@ -234,6 +330,11 @@ class DecoderEngine:
             t[slot:slot + 1].zero_()
         self.llm.token_log[slot].zero_()
 
+    def _paged_admission(self) -> bool:
+        """Admission takes pages from the pool (PagedKVCache.admit_prefix) with the prefix cache, and once a group has
+        been forked: slots then no longer hold their static table rows."""
+        return self.prefix_cache or self.llm.cache.shared
+
     def _admit(self, slot: int, request: Request, rows: torch.Tensor):
         """Prefix caching: digest the prompt's full pages (ops.page_digest), chain them into keys, take the cached
         pages of the longest run of hits and private pages for everything else the request can write
@@ -245,11 +346,12 @@ class DecoderEngine:
         from .model.mixtral import prefix_keys
         c = self.llm.cache
         S, ps = rows.shape[0], c.page_size
-        keys = prefix_keys(ops.page_digest(rows, ps).cpu())
+        keys = prefix_keys(ops.page_digest(rows, ps).cpu()) if self.prefix_cache else []
         n_pages = -(-(S + request.max_new_tokens + self.overrun) // ps)
         P = c.admit_prefix(slot, keys, S, n_pages)
-        self.prefix_stats["hit_pages"] += P // ps
-        self.prefix_stats["missed_pages"] += len(keys) - P // ps
+        if self.prefix_cache:
+            self.prefix_stats["hit_pages"] += P // ps
+            self.prefix_stats["missed_pages"] += len(keys) - P // ps
         c.cache_len[slot:slot + 1] = P
         return P, keys
 
@@ -264,9 +366,9 @@ class DecoderEngine:
         p = request.payload
         emb, lens = self.model._embeds_for(p["input_ids"], p.get("images"), p.get("audios"))
         self._check(request, int(lens[0]))
-        self.llm.sampling.set(slot, request.sampling, request.logprobs)
+        self.llm.sampling.set(slot, request.sampling, log_width(request))
         rows = emb[0, : lens[0]].contiguous()
-        P, keys = self._admit(slot, request, rows) if self.prefix_cache else (0, None)
+        P, keys = self._admit(slot, request, rows) if self._paged_admission() else (0, None)
         self.llm.prefill(rows[P:], slot=slot, sampled=request.sampling is not None, start=P,
                          logprobs=self.llm.sampling.log_width(slot, 1))
         if self.prefix_cache:
@@ -280,9 +382,9 @@ class DecoderEngine:
         emb, lens = self.model._embeds_for(p["input_ids"], p.get("images"), p.get("audios"))
         S = int(lens[0])
         self._check(request, S)
-        self.llm.sampling.set(slot, request.sampling, request.logprobs)
+        self.llm.sampling.set(slot, request.sampling, log_width(request))
         rows = emb[0, :S].contiguous()
-        if not self.prefix_cache:
+        if not self._paged_admission():
             self._adm = (rows, request.sampling is not None, self.llm.sampling.log_width(slot, 1))
             return S
         P, keys = self._admit(slot, request, rows)
@@ -315,10 +417,18 @@ class DecoderEngine:
         else:
             self.llm.decode_step_batched(n_active, use_graph=self.use_graph, sampled=sampled, logprobs=logprobs)
 
+    def fork(self, slot: int, count: int, max_new_tokens: int) -> None:
+        """Parallel sampling: the request just prefilled into `slot` continues as `count` sequences in slots
+        slot .. slot + count - 1 (MixtralDecoder.fork_sampled), each owning pages for its max_new_tokens + overrun
+        positions past the prompt."""
+        S = int(self.llm.cache.cache_len[slot])
+        n_pages = -(-(S + max_new_tokens + self.overrun) // self.llm.cache.page_size)
+        self.llm.fork_sampled(slot, count, S, n_pages)
+
     def swap(self, i: int, j: int) -> None:
         swap_rows(self._slot_tensors, i, j)
         if i != j:
-            if self.prefix_cache:                    # the host table rows follow block_table's
+            if self.llm.cache.shared:                # the host table rows follow block_table's
                 self.llm.cache.pool.swap(i, j)
             self.llm.sampling.swap(i, j)
             if self.llm.lp_log is not None:          # the logprob log rows move with their request

@@ -209,6 +209,30 @@ class PagePool:
                     self.refs[pg] += 1
         return self._private_write_pages([*dsts, src], length)     # src keeps its page
 
+    def fork_reserved(self, src: int, dsts: Sequence[int], length: int, n_pages: int) -> List[Tuple[int, int]]:
+        """Parallel sampling: dsts continue the `length` tokens of src and then advance on their own, so each owns, from
+        now on, private pages for everything it can write ([length, n_pages * page_size)), as admission guarantees a
+        fresh request.  They share src's full pages, take fresh pages (free ones, else evicted indexed ones: `_take`)
+        from page length // page_size up to n_pages, and the partial last page of src is copied into their first fresh
+        page.  src's row is left as it is; the dst rows' previous pages are released first.  Returns the (src, dst)
+        pages to copy.  Never fails: every row holds at most len(static row) pages, so the pages the dsts give up and
+        the unreferenced ones cover what they take."""
+        ps, full = self.page_size, length // self.page_size
+        assert src not in dsts and length < n_pages * ps and n_pages <= len(self.table[src])
+        for d in dsts:
+            self.release(d)
+        pairs = []
+        for d in dsts:
+            row = self.table[d]
+            for i in range(full):
+                row[i] = self.table[src][i]
+                self.refs[row[i]] += 1
+            for i in range(full, n_pages):
+                row[i] = self._take()
+            if length % ps:
+                pairs.append((self.table[src][full], row[full]))
+        return pairs
+
     def reorder(self, parents: Sequence[int], length: int) -> List[Tuple[int, int]]:
         """Slot i (i < len(parents)) continues slot parents[i], every slot holding `length` tokens: each takes its
         parent's row, then the page the next row lands in is made private (one child keeps the parent's page)."""
@@ -326,6 +350,17 @@ class PagedKVCache:
         self._share()
         self._apply(self.pool.fork(src, dsts, length))
 
+    def fork_reserved(self, src: int, dsts: Sequence[int], length: int, n_pages: int):
+        """PagePool.fork_reserved on the device tables: the dst rows of block_table and slot_map are written (a
+        reused slot prefills through slot_map) and the partial page is copied in one kv_copy_pages launch."""
+        self._share()
+        pairs = self.pool.fork_reserved(src, dsts, length, n_pages)
+        dsts = list(dsts)
+        rows = torch.tensor([self.pool.table[d] for d in dsts], dtype=torch.int32)
+        self.block_table[dsts] = rows.to(self.block_table.device)
+        self.slot_map[dsts] = self._slot_map_rows(rows).to(self.slot_map.device)
+        self._copy(pairs)
+
     def reorder(self, parents: Sequence[int], length: int):
         """PagePool.reorder on the device tables, with one kv_copy_pages launch for the pages it copies."""
         self._share()
@@ -333,6 +368,9 @@ class PagedKVCache:
 
     def _apply(self, pairs):
         self.block_table.copy_(torch.tensor(self.pool.table, dtype=torch.int32))
+        self._copy(pairs)
+
+    def _copy(self, pairs):
         if not pairs:
             return
         if self._layer_base is None:
@@ -776,12 +814,12 @@ class MixtralDecoder:
         sp, rows = self.sampling, slice(s0, s0 + n)
         if logprobs is None:
             ops.sample_rows(self.d_logits[rows], sp.temperature[rows], sp.top_k[rows], sp.top_p[rows], sp.seed[rows],
-                            self.gen_count[rows], self.best[rows], scores)
+                            self.gen_count[rows], self.best[rows], scores, streams=sp.stream[rows])
             return
         lg = self.enable_logprob_log()
         ops.sample_logprobs(self.d_logits[rows], sp.temperature[rows], sp.top_k[rows], sp.top_p[rows], sp.seed[rows],
                             self.gen_count[rows], self.best[rows], lg[0][rows], lg[1][rows], lg[2][rows], lg[3][rows],
-                            logprobs, scores=scores, log_softmax_scores=log_softmax_scores)
+                            logprobs, scores=scores, log_softmax_scores=log_softmax_scores, streams=sp.stream[rows])
 
     def enable_logprob_log(self):
         """Allocate the per-slot logprob log: (logprob f32 [B, R], rank i32 [B, R], top ids i32 [B, R, 20], top
@@ -825,6 +863,23 @@ class MixtralDecoder:
         for t in (c.cache_len, c.cur_pos, self.gen_count, self.token_log, self.best):
             t[idx] = t[src].clone()
         c.fork(src, dsts, length)
+
+    def fork_sampled(self, src: int, count: int, length: int, n_pages: int, scores: Optional[torch.Tensor] = None):
+        """Parallel sampling: slot src has just prefilled its `length` prompt rows with a sampled first token; slots
+        src + 1 .. src + count - 1 become further sampled sequences of the same request.  They share src's full KV
+        pages, get a copy of its partial page and private pages up to n_pages (PagedKVCache.fork_reserved), take its
+        sampler parameters with streams 1 .. count - 1 (SlotSampling.fork) and its decode state, and each draws its own
+        first token at counter 0 from src's last-row logits (with its logprob record when src's request asks).
+        `scores` (a per-slot score log [>= src + count, rows, V]): their warped rows land in row 0 of their slots."""
+        if count < 2:
+            return
+        c, dst = self.cache, slice(src + 1, src + count)
+        for t in (c.cache_len, c.cur_pos, self.gen_count, self.token_log, self.d_logits):
+            t[dst] = t[src].clone()
+        self.sampling.fork(src, count)
+        c.fork_reserved(src, range(src + 1, src + count), length, n_pages)
+        self._sample(src + 1, count - 1, scores[dst] if scores is not None else None,
+                     self.sampling.log_width(src, 1))
 
     def enable_score_log(self):
         """Allocate the per-step logits log (HF `output_scores=True`): row i holds the logits token i was chosen from.
@@ -871,11 +926,12 @@ class MixtralDecoder:
 
     # ------------------------------------------------------------------------------------------ batched decode
     def _batched_step_kernels(self, B: int, sampled: bool = False, logprobs: Optional[int] = None,
-                              scores: bool = False):
+                              scores: bool = False, warped_scores: bool = False):
         """One token for each of B sequences through the GEMM path (weights of every touched expert are streamed once
         for the whole batch; BASELINE configs[4]).  The prefill's layer loop with M = B rows at B different
         positions and the paged decode attention.  `scores` (with `logprobs`): the sampler also writes each slot's
-        log-softmax row to the beam score log."""
+        log-softmax row to the beam score log; `warped_scores` (sampled): each slot's warped row to the same per-slot
+        log (parallel sampling's output_scores)."""
         c, w, cache = self.cfg, self.w, self.cache
         h = self.d_h[:B]
         ops.decode_embed(self.best[:B], self.token_log[:B], self.gen_count[:B], cache.cache_len[:B], cache.cur_pos[:B],
@@ -887,7 +943,7 @@ class MixtralDecoder:
         xn = self.run_layers(h, cache.cur_pos[:B], slots, cache.k, cache.v, attention, final_norm=True)
         logits = ops.linear(xn, w["lm_head"], out=self.d_logits[:B])
         if sampled or logprobs is not None:   # greedy rows (temperature 0) get argmax_rows' word: a mixed batch keeps their tokens
-            self._sample(0, B, self.beam_scores if scores else None, logprobs, scores)
+            self._sample(0, B, self.beam_scores if (scores or warped_scores) else None, logprobs, scores)
         else:
             ops.argmax_rows(logits, self.best[:B])
 
@@ -897,17 +953,22 @@ class MixtralDecoder:
 
     @torch.no_grad()
     def decode_step_batched(self, B: int, use_graph: bool = True, sampled: bool = False,
-                            logprobs: Optional[int] = None, scores: bool = False):
-        """`scores`: write the log-softmax rows to the beam score log (enable_beam_score_log; needs `logprobs`)."""
+                            logprobs: Optional[int] = None, scores: bool = False, warped_scores: bool = False):
+        """`scores`: write the log-softmax rows to the beam score log (enable_beam_score_log; needs `logprobs`).
+        `warped_scores`: write the warped rows to that log instead (needs `sampled`)."""
         assert self.ep_world == 1 and 1 <= B <= self.max_batch
         assert not scores or (logprobs is not None and self.beam_scores is not None and self.beam_scores.shape[0] >= B)
-        step = lambda: self._batched_step_kernels(B, sampled, logprobs, scores)
+        assert not warped_scores or (sampled and not scores and self.beam_scores is not None
+                                     and self.beam_scores.shape[0] >= B)
+        step = lambda: self._batched_step_kernels(B, sampled, logprobs, scores, warped_scores)
         if not use_graph:
             step()
             return
         key = (B, sampled, "logprobs", logprobs) if logprobs is not None else (B, sampled)
         if scores:
             key += ("scores",)
+        if warped_scores:
+            key += ("scores", "warped")     # "scores": re-captured when the log grows (enable_beam_score_log)
         self._replay(self._bgraphs, key, step)   # one graph per batch size (continuous batching changes B)
 
     def _replay(self, graphs: dict, key, step):

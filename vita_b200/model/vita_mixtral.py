@@ -445,24 +445,53 @@ class VITAMixtralForCausalLM:
         `length_penalty`, `early_stopping` and `num_return_sequences` (vita_b200/beam.py).  `sequences` holds the best
         `num_return_sequences` hypotheses, padded with `eos_token_id`, with `sequences_scores` and `beam_indices`;
         `scores` (with `output_scores`) holds one [num_beams, V] block of the running beams' log-softmax rows per step.
-        The beams share their KV pages copy-on-write and advance together through the batched decode step."""
+        The beams share their KV pages copy-on-write and advance together through the batched decode step.
+
+        `do_sample=True` with `num_return_sequences` = N > 1 (at most the model's `max_batch`): N independent samples
+        of the prompt, as HF 4.41 returns them.  The prompt is prefilled once and its KV pages are shared by the N
+        sequences; sequence i draws from stream i of the call's key, so sequence 0 starts with the token the call with
+        one sequence draws.  `sequences` is [N, L + T], T the longest row; a row is finished at its EOS or when a
+        stopping criterion marks it (a bool result marks every row), and finished rows are padded with
+        `eos_token_id`.  `scores` holds one [N, V] block of warped rows per step, `logprobs` one tuple of
+        TokenLogprobs per sequence."""
         if num_beams != 1:
             return self._beam_search(input_ids, images, audios, num_beams, num_return_sequences, length_penalty,
                                      early_stopping, do_sample, logprobs, output_scores, return_dict_in_generate,
                                      max_new_tokens, stopping_criteria, eos_token_id, use_graph)
+        N = num_return_sequences
+        if isinstance(N, bool) or not isinstance(N, int) or N < 1:
+            raise ValueError(f"num_return_sequences has to be a positive integer, got {N!r}")
         params = from_hf(do_sample, temperature, top_k, top_p, seed, **kw)
         sampled = params is not None
+        if N > 1 and not sampled:
+            raise ValueError(f"greedy decoding without beam search does not support num_return_sequences different "
+                             f"than 1 (got {N})")
         n_top = check_logprobs(logprobs)
         want_lp = n_top is not None
         if sampled and self.llm.ep_world > 1:
             raise ValueError("sampled decoding is single-GPU (the expert-parallel mode serves greedy requests)")
         if want_lp and self.llm.ep_world > 1:
             raise ValueError("logprobs are single-GPU (the expert-parallel mode serves greedy requests)")
+        if N > self.llm.max_batch:
+            raise ValueError(f"num_return_sequences={N} exceeds the model's max_batch ({self.llm.max_batch}): the "
+                             f"sequences run in decoder slots; build the model with max_batch >= {N}")
         if input_ids.shape[0] != 1:
             raise ValueError("generate() is single-sequence like the demo; use generate_batch() for more")
+        if N > 1 and max_new_tokens < 1:
+            raise ValueError("num_return_sequences > 1 needs max_new_tokens >= 1")
         emb, lens = self._embeds_for(input_ids, images, audios)
         llm = self.llm
         llm.check_capacity(lens[0], max_new_tokens)
+        if N > 1:
+            llm.reset()
+            try:
+                return self._run_samples(emb[0, : lens[0]].contiguous(), input_ids, N, params, n_top, output_scores,
+                                         return_dict_in_generate, max_new_tokens, stopping_criteria, eos_token_id,
+                                         use_graph, sync_every)
+            finally:
+                llm.cache.unshare()      # the static slot tables again, a full pool, greedy slots on stream 0
+                for b in range(N):
+                    llm.sampling.set(b, None)
         llm.reset()
         llm.sampling.set(0, params, n_top)
         width = llm.sampling.log_width(0, 1)                  # top entries the logprob log records (None: no log)
@@ -503,6 +532,62 @@ class VITAMixtralForCausalLM:
             return seq
         scores = tuple(score_log[i: i + 1] for i in range(n_new)) if output_scores else None
         lps = tuple(llm.read_logprobs(0, seq_host[0, L: L + n_new].tolist(), n_top)) if want_lp else None
+        return GenerateOutput(seq, scores, lps)
+
+    def _run_samples(self, emb, input_ids, N, params, n_top, output_scores, return_dict_in_generate, max_new_tokens,
+                     stopping_criteria, eos_token_id, use_graph, sync_every):
+        """generate(do_sample=True, num_return_sequences=N > 1), HF 4.41's `_sample` loop over the prompt expanded N
+        times: prefill into slot 0, fork it into slots 1 .. N - 1 (MixtralDecoder.fork_sampled), then one batched
+        step for all N per token.  Tokens are read back every `sync_every` steps; the stopping rules then run once per
+        step on the [N, L + i + 1] view, in which finished rows hold the pad id."""
+        llm = self.llm
+        S = emb.shape[0]
+        llm.sampling.set(0, params, n_top)
+        width = llm.sampling.log_width(0, 1)
+        score_log = llm.enable_beam_score_log(N, max_new_tokens) if output_scores else None
+        if width is not None:
+            llm.enable_logprob_log()
+        llm.prefill(emb, slot=0, sampled=True, scores=score_log[0] if output_scores else None, logprobs=width)
+        llm.fork_sampled(0, N, S, -(-(S + max_new_tokens) // llm.cache.page_size), score_log)
+        prompt = input_ids[0].tolist()
+        L, pad = len(prompt), eos_token_id               # HF pads with eos_token_id when no pad id is given
+        seq_host = torch.empty(N, L + max_new_tokens, dtype=torch.long)
+        seq_host[:, :L] = torch.tensor(prompt, dtype=torch.long)
+        finished = torch.zeros(N, dtype=torch.bool)
+        ends = [max_new_tokens] * N                      # tokens of each row before its padding
+        t = step = 0
+        while t < max_new_tokens and not bool(finished.all()):
+            n = min(sync_every, max_new_tokens - step)
+            for _ in range(n):
+                llm.decode_step_batched(N, use_graph=use_graph, sampled=True, logprobs=width,
+                                        warped_scores=output_scores)
+            step += n
+            t0, new = t, llm.token_log[:N, t:step].to("cpu", torch.long)   # one host sync per `sync_every` tokens
+            for i in range(t0, step):
+                col = new[:, i - t0].clone()
+                if pad is not None:
+                    col[finished] = pad
+                seq_host[:, L + i] = col
+                was = finished.clone()
+                if eos_token_id is not None:
+                    finished |= col == eos_token_id
+                if stopping_criteria:
+                    view = seq_host[:, : L + i + 1]
+                    for sc in stopping_criteria:
+                        finished |= torch.as_tensor(sc(view, None), dtype=torch.bool).reshape(-1).expand(N)
+                for b in torch.nonzero(finished & ~was).flatten().tolist():
+                    ends[b] = i + 1
+                t = i + 1
+                if bool(finished.all()):
+                    break
+        seq = seq_host[:, : L + t].to(input_ids.device)
+        if not return_dict_in_generate:
+            return seq
+        scores = tuple(score_log[:N, i] for i in range(t)) if output_scores else None
+        lps = None
+        if n_top is not None:                           # without a pad id a finished row keeps its tokens
+            lps = tuple(tuple(llm.read_logprobs(b, seq_host[b, L: L + (min(ends[b], t) if pad is not None else t)]
+                                                .tolist(), n_top)) for b in range(N))
         return GenerateOutput(seq, scores, lps)
 
     @torch.no_grad()

@@ -286,11 +286,19 @@ def argmax_rows(logits, best):
     _lib.call("vita_argmax_rows", _p(logits), _p(best), logits.shape[0], logits.shape[1], _stream())
 
 
-def sample_rows(logits, temperature, top_k, top_p, seed, counter, best, scores: Optional[torch.Tensor] = None):
+def _chk_streams(streams, B: int, name: str):
+    if streams is not None:
+        _chk(streams, torch.int32, "streams")
+        if streams.numel() < B:
+            raise _lib.VitaB200Error(f"{name}: streams has fewer than {B} rows")
+
+
+def sample_rows(logits, temperature, top_k, top_p, seed, counter, best, scores: Optional[torch.Tensor] = None,
+                streams: Optional[torch.Tensor] = None):
     """Sampled next token per row into the packed arg-max words `best` (contract: vita_b200/sampling.py).
     logits [B, V] bf16 (rows may be strided); temperature / top_p f32 [B], top_k / counter i32 [B], seed i64 [B]
     (the 64-bit Philox key, bit pattern); scores [B, rows, V] or [rows, V] (B = 1) bf16: row counter[b] receives
-    the warped logits."""
+    the warped logits.  streams (i32 [B], optional; None = stream 0): the stream index of each row's draw."""
     _chk(logits, BF16, "logits", contiguous=False); _chk(best, torch.int64, "best")
     _chk(temperature, torch.float32, "temperature"); _chk(top_p, torch.float32, "top_p")
     _chk(top_k, torch.int32, "top_k"); _chk(counter, torch.int32, "counter"); _chk(seed, torch.int64, "seed")
@@ -309,20 +317,22 @@ def sample_rows(logits, temperature, top_k, top_p, seed, counter, best, scores: 
         if scores.shape[0] < B or scores.shape[2] != V:
             raise _lib.VitaB200Error("sample_rows: scores must be [B, rows, V]")
         rows = scores.shape[1]
-    _lib.call("vita_sample_rows", _p(logits), logits.stride(0), B, V, _p(temperature), _p(top_k), _p(top_p),
-              _p(seed), _p(counter), _p(best), _p(scores), V, rows, _stream())
+    _chk_streams(streams, B, "sample_rows")
+    _lib.call("vita_sample_rows_streams", _p(logits), logits.stride(0), B, V, _p(temperature), _p(top_k), _p(top_p),
+              _p(seed), _p(counter), _p(streams), None, _p(best), _p(scores), V, rows, None, None, None, None, 0, 0,
+              0, 0, _stream())
 
 
 def sample_logprobs(logits, temperature, top_k, top_p, seed, counter, best, logprob, rank, top_ids, top_logprobs,
                     n_top: int, target: Optional[torch.Tensor] = None, scores: Optional[torch.Tensor] = None,
-                    log_softmax_scores: bool = False):
+                    log_softmax_scores: bool = False, streams: Optional[torch.Tensor] = None):
     """`sample_rows` plus log-probabilities over the processed row (contract: vita_b200/sampling.py).
     `target` (i32 [B], optional): rows with target[b] in [0, V) score that token and draw nothing (best[b] gets the
     greedy word); the other rows score the token they choose.  Outputs: logprob f32 / rank i32 of shape [B] (row b) or
     [B, rows] (row counter[b] of request b, a device-resident log); top_ids i32 / top_logprobs f32 of that shape plus
     a last dimension >= n_top (0 <= n_top <= 20): the n_top largest logits, lowest index first on ties.
     `log_softmax_scores`: the score rows receive bf16(logprob) of every token (HF beam search's scores) instead of the
-    processed row."""
+    processed row.  `streams` as for `sample_rows`."""
     _chk(logits, BF16, "logits", contiguous=False); _chk(best, torch.int64, "best")
     _chk(temperature, torch.float32, "temperature"); _chk(top_p, torch.float32, "top_p")
     _chk(top_k, torch.int32, "top_k"); _chk(counter, torch.int32, "counter"); _chk(seed, torch.int64, "seed")
@@ -356,11 +366,11 @@ def sample_logprobs(logits, temperature, top_k, top_p, seed, counter, best, logp
         if scores.shape[0] < B or scores.shape[2] != V:
             raise _lib.VitaB200Error("sample_logprobs: scores must be [B, rows, V]")
         rows = scores.shape[1]
-    entry = "vita_sample_rows_logsoftmax" if log_softmax_scores else "vita_sample_rows_logprobs"
-    _lib.call(entry, _p(logits), logits.stride(0), B, V, _p(temperature), _p(top_k), _p(top_p),
-              _p(seed), _p(counter), _p(target), _p(best), _p(scores), V, rows, _p(logprob), _p(rank),
+    _chk_streams(streams, B, "sample_logprobs")
+    _lib.call("vita_sample_rows_streams", _p(logits), logits.stride(0), B, V, _p(temperature), _p(top_k), _p(top_p),
+              _p(seed), _p(counter), _p(streams), _p(target), _p(best), _p(scores), V, rows, _p(logprob), _p(rank),
               _p(top_ids) if n_top > 0 else None, _p(top_logprobs) if n_top > 0 else None, int(n_top), top_ld,
-              out_rows, _stream())
+              out_rows, int(log_softmax_scores), _stream())
 
 
 def kv_copy_pages(layer_base: torch.Tensor, pairs: torch.Tensor, n_pages: int, page_bytes: int):

@@ -1,8 +1,13 @@
 """Sampled decoding: the one place that maps generation parameters to the per-row sampler parameters.
 
 The kernel (csrc/sample.cu, `ops.sample_rows`) takes, per row, `temperature` (0 = greedy), `top_k` (<= 0: off),
-`top_p` (>= 1: off), a 64-bit Philox key `seed`, and the index `n` of the token being drawn within its request (the
-decoder passes its device-resident `gen_count`, so a request draws the same tokens in any slot, batch or graph).
+`top_p` (>= 1: off), a 64-bit Philox key `seed`, the index `n` of the token being drawn within its request (the
+decoder passes its device-resident `gen_count`, so a request draws the same tokens in any slot, batch or graph), and a
+stream index `s`: the noise of token n comes from Philox counter (r >> 2, n, s, 0).
+
+Parallel sampling (`generate(do_sample=True, num_return_sequences=N)`, `Request.n` / `Request.best_of`): the N
+sequences of one request share its key and draw from streams 0 .. N-1 (`SlotSampling.fork`), so they are independent
+samples, reproducible from one seed, and sequence 0 draws exactly what the same request with one sequence draws.
 
 Warping follows HF transformers 4.41 (`TemperatureLogitsWarper` -> `TopKLogitsWarper` -> `TopPLogitsWarper`, the
 version the reference pins), which is also what vLLM does: x = l / T in fp32 from the bf16 logits; top-k keeps every
@@ -179,15 +184,16 @@ class SlotSampling:
         self.top_k = torch.zeros(max_batch, dtype=torch.int32, device=dev)
         self.top_p = torch.ones(max_batch, dtype=torch.float32, device=dev)
         self.seed = torch.zeros(max_batch, dtype=torch.int64, device=dev)
+        self.stream = torch.zeros(max_batch, dtype=torch.int32, device=dev)  # stream index of the slot's sequence
         self.sampled: List[bool] = [False] * max_batch
         self.logprobs: List[Optional[int]] = [None] * max_batch     # top-N a slot's request asked for (None: none)
 
     @property
     def tensors(self):
-        return [self.temperature, self.top_k, self.top_p, self.seed]
+        return [self.temperature, self.top_k, self.top_p, self.seed, self.stream]
 
     def set(self, slot: int, params: Optional[SamplingParams], logprobs: Optional[int] = None) -> None:
-        """params None = greedy; `logprobs` = the request's top-N (None: no logprobs)."""
+        """params None = greedy; `logprobs` = the request's top-N (None: no logprobs).  The slot draws from stream 0."""
         self.logprobs[slot] = check_logprobs(logprobs)
         p = params or SamplingParams(1.0)
         row = slice(slot, slot + 1)
@@ -195,7 +201,17 @@ class SlotSampling:
         self.top_k[row] = p.top_k
         self.top_p[row] = p.top_p
         self.seed[row] = _i64(p.seed)
+        self.stream[row] = 0
         self.sampled[slot] = params is not None
+
+    def fork(self, src: int, count: int) -> None:
+        """Slots src + 1 .. src + count - 1 take the parameters of slot src (stream 0) with streams 1 .. count - 1."""
+        dst = slice(src + 1, src + count)
+        for t in (self.temperature, self.top_k, self.top_p, self.seed):
+            t[dst] = t[src].clone()
+        self.stream[dst] = torch.arange(1, count, dtype=torch.int32, device=self.stream.device)
+        for i in range(src + 1, src + count):
+            self.sampled[i], self.logprobs[i] = self.sampled[src], self.logprobs[src]
 
     def swap(self, i: int, j: int) -> None:
         self.sampled[i], self.sampled[j] = self.sampled[j], self.sampled[i]
