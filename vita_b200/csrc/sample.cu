@@ -20,8 +20,9 @@
 // rows, x_r over the kept set and -inf outside it otherwise --
 //   logprob(r) = x_r - x_max - log(Z * 2^-40), Z = sum over the kept set of the fixed-point masses above (u64);
 //   rank(r) = 1 + #{kept tokens with a strictly greater logit}; top-N = the N largest logits, lowest index first on
-//   ties (the N-th largest comes from the same radix selection as top-k, with k = N).  Both compare the ordered keys
-//   with -0.0 read as +0.0, so equal logits are equal.
+//   ties (the N-th largest comes from the same radix selection as top-k, with k = N).
+// Every comparison of logits -- the top-k and top-p thresholds, the kept test, ranks and top-N -- reads the ordered
+// keys with -0.0 as +0.0 (canon_key), so equal logits are equal: -0.0 and +0.0 are kept or dropped together.
 // A row with a target id scores that token and draws nothing (prompt rows: the next prompt token).
 // The LSM variant (vita_sample_rows_logsoftmax) writes bf16(logprob(r)) of every token to the score row instead of the
 // processed row: HF beam search's per-step scores, from the same Z as the logprob.
@@ -97,13 +98,13 @@ __device__ __forceinline__ unsigned long long block_max_u64(unsigned long long v
     return red[0];
 }
 
-// -0.0 and +0.0 are one value to ranks and top-N: the key of -0.0 (0x7FFF) is read as that of +0.0
+// -0.0 and +0.0 are one value: the key of -0.0 (0x7FFF) is read as that of +0.0
 __device__ __forceinline__ uint32_t canon_key(uint32_t k) { return k == 0x7FFFu ? 0x8000u : k; }
 
-// Histogram over the keys >= floor_key: high bytes (hi_bin < 0) or the low bytes of the keys whose high byte is
-// hi_bin.  Weight 1 (counts) or the fixed-point mass exp(x - x_max) * 2^40.  Result in tot[256].
-// CANON (counts only): over canon_key(key), with the lanes of a warp that hit one bin adding once.
-template <bool CANON = false>
+// Histogram over the canonical keys >= floor_key: high bytes (hi_bin < 0) or the low bytes of the keys whose high
+// byte is hi_bin.  Weight 1 (counts) or the fixed-point mass exp(x - x_max) * 2^40.  Result in tot[256].
+// WARP_MATCH (counts only, no floor): the lanes of a warp that hit one bin add once.
+template <bool WARP_MATCH = false>
 __device__ void sample_hist(const uint16_t* keys, int V, unsigned long long* whist, unsigned long long* tot,
                             int hi_bin, uint32_t floor_key, bool mass, float T, float x_max) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -111,7 +112,7 @@ __device__ void sample_hist(const uint16_t* keys, int V, unsigned long long* whi
 #pragma unroll
     for (int j = 0; j < 8; ++j) h[lane + 32 * j] = 0ull;
     __syncwarp();
-    if constexpr (CANON) {
+    if constexpr (WARP_MATCH) {
         // every lane runs every iteration (the bound is uniform), so the whole warp takes part in the match
         for (int base = 0; base < V; base += kSampleThreads) {
             const int i = base + static_cast<int>(threadIdx.x);
@@ -124,8 +125,8 @@ __device__ void sample_hist(const uint16_t* keys, int V, unsigned long long* whi
             if (bin >= 0 && lane == __ffs(peers) - 1) atomicAdd(h + bin, static_cast<unsigned long long>(__popc(peers)));
         }
     }
-    for (int i = threadIdx.x; i < V && !CANON; i += kSampleThreads) {
-        const uint32_t k = keys[i];
+    for (int i = threadIdx.x; i < V && !WARP_MATCH; i += kSampleThreads) {
+        const uint32_t k = canon_key(keys[i]);
         if (k < floor_key) continue;
         if (hi_bin >= 0 && static_cast<int>(k >> 8) != hi_bin) continue;
         unsigned long long wt = 1ull;
@@ -216,7 +217,8 @@ __device__ __forceinline__ float key_x(uint32_t k, float T) {
     else return key_value(k);
 }
 
-// Logprob, rank and top-N of token `idx` over the processed row (kept set = keys >= thr).  Every thread calls it.
+// Logprob, rank and top-N of token `idx` over the processed row (kept set = staged keys >= thr).  Every thread
+// calls it.
 // LSM: srow (may be null) receives the log-softmax of the whole processed row.
 template <bool SCALED, bool LSM>
 __device__ void write_logprobs(const uint16_t* keys, int V, uint32_t thr, float T, float x_max, int idx,
@@ -380,10 +382,7 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
         if constexpr (!LOGPROBS) return;
     }
     const uint32_t ord = static_cast<uint32_t>(arg >> 32);     // undo pack_score's float ordering, then re-key
-    // max_key is the lowest staged key of the largest value: the thresholds below compare it with the raw keys, on
-    // which -0.0 (0x7FFF) sorts just below +0.0 (0x8000), and a maximum of zero has to keep both zeros
-    const uint32_t max_canon = bf16_key(((ord & 0x80000000u) ? (ord & 0x7FFFFFFFu) : ~ord) >> 16);
-    const uint32_t max_key = max_canon == 0x8000u ? 0x7FFFu : max_canon;
+    const uint32_t max_key = bf16_key(((ord & 0x80000000u) ? (ord & 0x7FFFFFFFu) : ~ord) >> 16);   // canonical
     if constexpr (LOGPROBS) {
         if (greedy) {                                    // the processed row is the logits: x = l, every token kept
             const int idx = tgt >= 0 ? tgt : static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(arg & 0xFFFFFFFFull));
@@ -394,7 +393,7 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
     }
     const float x_max = __fdiv_rn(key_value(max_key), T);
 
-    // top-k threshold: the k-th largest key
+    // top-k threshold: the k-th largest canonical key
     uint32_t thr = 0u;
     if (k > 0 && k < V) {
         sample_hist(keys, V, whist, tot, -1, 0u, false, T, x_max);
@@ -407,7 +406,8 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
         __syncthreads();
         thr = (static_cast<uint32_t>(hb) << 8) | static_cast<uint32_t>(s_bin);
     }
-    // top-p threshold over the top-k survivors: the lowest key whose strictly-greater survivor mass is < p * Z
+    // top-p threshold over the top-k survivors: the lowest canonical key whose strictly-greater survivor mass is
+    // < p * Z
     if (p < 1.0f) {
         sample_hist(keys, V, whist, tot, -1, thr, true, T, x_max);
         if (tid < 32) {                                  // Z = survivor mass = sum of all bins
@@ -433,6 +433,9 @@ sample_rows_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V
         }
         thr = tp > thr ? tp : thr;
     }
+    // the thresholds are canonical keys; the kept tests below read the staged keys, on which -0.0 (0x7FFF) sorts
+    // just below +0.0 (0x8000): a threshold at zero is lowered to -0.0's key so that both zeros are kept
+    if (thr == 0x8000u) thr = 0x7FFFu;
 
     // Gumbel-max over the kept keys (>= thr)
     const float x_floor = x_max - kGumbelPrune;
