@@ -439,9 +439,13 @@ class LayerAttention:
 class MixtralDecoder:
     def __init__(self, cfg: LLMConfig, weights: dict, device, max_batch: int = 1, max_seq_len: Optional[int] = None,
                  max_new_tokens: int = 1024, page_size: int = 16, decode_splits: int = 16, shuffle_pages: bool = False,
-                 kv_cache_dtype: str = "auto", k_scale=1.0, v_scale=1.0):
+                 kv_cache_dtype: str = "auto", k_scale=1.0, v_scale=1.0,
+                 ep_alloc: Optional[Callable[[int], Tuple[torch.Tensor, List[int]]]] = None):
         """`kv_cache_dtype`: "auto" / "bf16" (default) or "fp8" / "fp8_e4m3", an e4m3 paged KV cache at half the bytes
-        with per-layer `k_scale` / `v_scale` (a float or one per layer; vLLM's defaults are 1.0)."""
+        with per-layer `k_scale` / `v_scale` (a float or one per layer; vLLM's defaults are 1.0).
+        `ep_alloc(nbytes) -> (own zeroed uint8 buffer, [base address of every rank's buffer])`: where the
+        sequence-sharded expert-parallel prefill gets its symmetric memory; default: NVLink symmetric memory over the
+        default process group (`_symm_alloc`)."""
         self.cfg = cfg
         self.w = weights
         self.device = torch.device(device)
@@ -465,7 +469,7 @@ class MixtralDecoder:
         storage = None
         if self.ep_mode == "seq":
             assert max_batch == 1 and not shuffle_pages, "sequence-sharded EP serves one sequence with in-order pages"
-            storage = self._init_ep_seq(page_rounded)
+            storage = self._init_ep_seq(page_rounded, ep_alloc or self._symm_alloc)
         self.cache = PagedKVCache(cfg, max_batch, max_seq_len, device, page_size, shuffle_pages, storage,
                                   kv_cache_dtype, k_scale, v_scale)
         self.max_new_tokens = max_new_tokens
@@ -515,12 +519,26 @@ class MixtralDecoder:
         self.e_lo, self.e_hi = self.ep_rank * per, (self.ep_rank + 1) * per
         assert weights["layers"][0]["w13"].shape[0] == per, "expert tensors do not match the EP layout"
 
-    def _init_ep_seq(self, S_max: int):
-        """One NVLink symmetric allocation for the sequence-sharded expert-parallel prefill: receive slots of the
-        combine, residual stream / normed rows (own tokens), the all-gathered post-attention activations with their
-        routing records, epoch flags, and the K/V pages of every layer.  Returns the page-storage callback."""
+    def _symm_alloc(self, nbytes: int):
+        """NVLink symmetric memory over the default process group: (own zeroed uint8 buffer, base address of every
+        rank's buffer), returned once every rank has zeroed its buffer."""
         import torch.distributed as dist
         import torch.distributed._symmetric_memory as symm_mem
+        sym = symm_mem.empty(nbytes, dtype=torch.uint8, device=self.device)
+        sym.zero_()
+        torch.cuda.synchronize()
+        hdl = symm_mem.rendezvous(sym, dist.group.WORLD)
+        delta = sym.data_ptr() - int(hdl.buffer_ptrs[hdl.rank])
+        bases = [int(p) + delta for p in hdl.buffer_ptrs]
+        assert hdl.world_size == self.ep_world and hdl.rank == self.ep_rank
+        self._symm_hdl = hdl
+        dist.barrier()
+        return sym, bases
+
+    def _init_ep_seq(self, S_max: int, alloc: Callable[[int], Tuple[torch.Tensor, List[int]]]):
+        """One symmetric allocation (`alloc`, see __init__) for the sequence-sharded expert-parallel prefill: receive
+        slots of the combine, residual stream / normed rows (own tokens), the all-gathered post-attention activations
+        with their routing records, epoch flags, and the K/V pages of every layer.  Returns the page-storage callback."""
         c, N, dev = self.cfg, self.ep_world, self.device
         H, L = c.hidden_size, c.num_hidden_layers
         kv_row = c.num_key_value_heads * c.head_dim * 2                       # bytes of one K (or V) row
@@ -532,26 +550,20 @@ class MixtralDecoder:
         offs = [0]
         for z in sizes:
             offs.append(offs[-1] + z)
-        sym = symm_mem.empty(offs[-1], dtype=torch.uint8, device=dev)
-        sym.zero_()
-        torch.cuda.synchronize()
-        hdl = symm_mem.rendezvous(sym, dist.group.WORLD)
-        delta = sym.data_ptr() - int(hdl.buffer_ptrs[hdl.rank])
-        bases = [int(p) + delta for p in hdl.buffer_ptrs]
-        assert hdl.world_size == N and hdl.rank == self.ep_rank
+        sym, bases = alloc(offs[-1])
+        assert sym.dtype == torch.uint8 and sym.numel() == offs[-1] and len(bases) == N
         off = dict(zip(names, offs))
         view = lambda n, dt: sym[off[n]:off[n] + sizes[names.index(n)]].view(dt)
         ptrs = lambda n: torch.tensor([b + off[n] for b in bases], dtype=torch.int64, device=dev)
         kv_layer = al(S_max * kv_row)
         self.ep_p2p = dict(
-            sym=sym, hdl=hdl, chunk_max=chunk_max, off=off, kv_layer=kv_layer, kv_row=kv_row,
+            sym=sym, chunk_max=chunk_max, off=off, kv_layer=kv_layer, kv_row=kv_row,
             base_ptrs=torch.tensor(bases, dtype=torch.int64, device=dev),
             rs=view("rs", BF16), h=view("h", BF16)[:S_max * H].view(S_max, H),
             xn=view("xn", BF16)[:S_max * H].view(S_max, H), xn2=view("xn2", BF16)[:S_max * H].view(S_max, H),
             ids=view("ids", torch.int32)[:S_max * 2].view(S_max, 2),      # (the regions are padded to 256 bytes)
             tw=view("tw", torch.float32)[:S_max * 2].view(S_max, 2), flags=view("flags", torch.int32),
             rs_ptrs=ptrs("rs"), h_ptrs=ptrs("h"), xn_ptrs=ptrs("xn"), flag_ptrs=ptrs("flags"), epoch=0)
-        dist.barrier()
 
         def storage(layer, which, shape):
             assert shape[0] == S_max, "K/V pages of the sequence-sharded prefill: one sequence, in-order pages"
@@ -696,6 +708,18 @@ class MixtralDecoder:
              the owner sums its two slots into the residual stream and applies the next RMSNorm.
         No partial sums anywhere: logits are bit-identical to the single-GPU model.  Returns the logits of the OWN rows
         when `all_logits`, the last-row logits on the rank that owns the last token otherwise (None elsewhere)."""
+        steps = self._prefill_ep_seq_steps(inputs_embeds, slot, all_logits, want_last_logits)
+        while True:
+            try:
+                next(steps)
+            except StopIteration as done:
+                return done.value
+
+    @torch.no_grad()
+    def _prefill_ep_seq_steps(self, inputs_embeds, slot, all_logits, want_last_logits):
+        """_prefill_ep_seq as a generator that yields right after each ep_signal (three times per layer, before the
+        wait that needs the other ranks' flags), so that one process can step several ranks on one device in turn.
+        Returns what _prefill_ep_seq returns."""
         assert slot == 0
         c, w, sy = self.cfg, self.w, self.ep_p2p
         S, H = inputs_embeds.shape
@@ -728,6 +752,7 @@ class MixtralDecoder:
                 ko = off["kv"] + 2 * li * kvl + t0 * kvr
                 ops.ep_push(sy["base_ptrs"], [(ko, n * kvr), (ko + kvl, n * kvr)], N, r)
             ops.ep_signal(sy["flag_ptrs"], 2, N, r, ep)
+            yield
             ops.ep_wait(sy["flags"], 2, N, ep, n_wait=r)          # K/V rows of the ranks before this one
             if n:
                 ops.attention(qkv, self.cache.k[li], self.cache.v[li], attn, (0, W, D), (0, nkv * D, D),
@@ -738,12 +763,14 @@ class MixtralDecoder:
                 ops.ep_push(sy["base_ptrs"], [(off["xn2"] + t0 * H * 2, n * H * 2), (off["ids"] + t0 * 8, n * 8),
                                               (off["tw"] + t0 * 8, n * 8)], N, r)
             ops.ep_signal(sy["flag_ptrs"], 3, N, r, ep)
+            yield
             ops.ep_wait(sy["flags"], 3, N, ep)
             ops.moe_align(ids, tw, ws["offs"], perm, rtok, rw, S, E, row_assign=ws["rassign"][:2 * S])
             ops.row_copy(xn2, rtok, None, xp, 2 * S)
             ops.moe_gate_up(xp, lw["w13"], act, offs_local, 2 * S)
             ops.moe_down_ep(act, lw["w2"], offs_local, rw, ws["rassign"][:2 * S], sy["rs_ptrs"], 2 * S, chunk)
             ops.ep_signal(sy["flag_ptrs"], 0, N, r, ep)
+            yield
             nxt = layers[li + 1]["ln1"] if li + 1 < len(layers) else (w["norm"] if all_logits else None)
             # (waits for flags[0] of every rank: all expert rows of the own tokens have landed)
             ops.ep_reduce_norm_gather(sy["rs"], sy["flags"], sy["h_ptrs"], sy["xn_ptrs"], nxt, t0, n, N, r, ep, H,
